@@ -40,11 +40,13 @@ SEED = 1234
 METRIC = "Mpixels/s scale+dither+sixel-encode @4K→cell"     # BASELINE.json "metric", first clause
 QUARTER, FAST_SCALE = 1, 8
 
-# name: source size, CalcScaleToFitDisplay arguments (width px, height px, cell_x, cell_y, width_stretch), canvas
+# name: source size, CalcScaleToFitDisplay arguments (width px, height px, cell_x, cell_y, width_stretch), canvas.
+# C2's batch is one frame per SM of an H100 SXM (132): its palette and dither kernels run one CTA per frame, so a
+# 133rd frame would start a second wave.
 CONFIGS = {
     "C1": dict(iw=640, ih=480, fit=(80, 50, 1, 2, 1.0), canvas="half", flags=0, animation=0, kind="alpha", frames=4096,
                text="C1: 640x480 RGBA -> -p half, 80x25 cells -> 67x50 -> half-block pick + ANSI emit"),
-    "C2": dict(iw=3840, ih=2160, fit=(2700, 1800, 9, 18, 1.0), canvas="sixel", flags=0, animation=0, kind="photo", frames=148,
+    "C2": dict(iw=3840, ih=2160, fit=(2700, 1800, 9, 18, 1.0), canvas="sixel", flags=0, animation=0, kind="photo", frames=132,
                text="C2: 3840x2160 RGBA -> -p sixel, 300x100 cells of 9x18px -> 2700x1519 (+pad 1524) Mitchell scale + compose + "
                     "256-colour median cut + FS dither + sixel"),
     "C3": dict(iw=1920, ih=1080, fit=(320, 100, 2, 2, 2.0), canvas="quarter", flags=QUARTER, animation=1, kind="video", frames=300,
@@ -125,7 +127,28 @@ def peak_hbm():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 700 W part)"
+
+
+DUMP_SAMPLE = 8 << 20      # encoded bytes kept by --dump-outputs when a step encodes more (32 MB as float32)
+
+
+def dump_outputs(d, out, offs):
+    """What one step returns to its caller, as .npy files in d: the frame offsets into the encoded byte stream
+    (offsets.npy, n_frames + 1, float64) and the bytes themselves as float32 -- all of them (encoded.npy), or,
+    when there are more than DUMP_SAMPLE, the bytes at DUMP_SAMPLE sorted positions drawn with a fixed seed
+    from [0, total) (encoded_sample.npy)."""
+    import torch
+    os.makedirs(d, exist_ok=True)
+    offs = offs.cpu().numpy()
+    total = int(offs[-1])
+    np.save(os.path.join(d, "offsets.npy"), offs.astype(np.float64))
+    if total <= DUMP_SAMPLE:
+        np.save(os.path.join(d, "encoded.npy"), out[:total].cpu().numpy().astype(np.float32))
+    else:
+        pos = np.sort(np.random.default_rng(SEED).integers(0, total, DUMP_SAMPLE))
+        sample = out[torch.from_numpy(pos).to(out.device)].cpu().numpy()
+        np.save(os.path.join(d, "encoded_sample.npy"), sample.astype(np.float32))
 
 
 # --------------------------------------------------------------------------- CPU reference arm
@@ -238,6 +261,9 @@ def main():
                     help="N>1: gather through torch.distributed point-to-point (round 1) instead of the C-ABI b200timg_gather")
     ap.add_argument("--exact-scale", action="store_true",
                     help="bit-exact scaler arithmetic on the sixel path instead of the <= 1 LSB fused-multiply-add mode")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="after the timed steps, write what the last one returned (frame offsets and encoded bytes) "
+                         "to DIR/*.npy (rank 0)")
     args = ap.parse_args()
     name, cfg = args.config, CONFIGS[args.config]
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
@@ -251,8 +277,7 @@ def main():
         return
 
     numa = pin_to_gpu_numa(local_rank)
-    # (NCCL's defaults are left alone: routing the point-to-point gather through the copy engines with
-    # NCCL_P2P_USE_CUDA_MEMCPY=1 measured 18.1 ms per step on 2 GPUs against 14.25 ms with NCCL's own NVLink kernels, run r2n3)
+    # (NCCL's defaults are left alone: its own NVLink kernels carry the point-to-point gather)
     import torch
     import torch.distributed as dist
     import timg_b200
@@ -365,6 +390,9 @@ def main():
     ms_total = e0.elapsed_time(e1)
     launches = ctx.launches - launches0
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        last = (step_no[0] - 1) % nbuf
+        dump_outputs(args.dump_outputs, outs[last], offss[last])
     t = torch.tensor([ms_total], dtype=torch.float64, device=dev)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -388,14 +416,8 @@ def main():
         alg_bytes = F * frame_bytes + total_bytes + (4 * ow * oh * (F - 1) if cfg["animation"] else 0)
         peak, how = peak_hbm()
         achieved = alg_bytes / (ms / n / 1e3) / 1e9
-        traffic = None       # dram__bytes_read+write of that kernel per launch, from the committed ncu capture
-        tp = os.path.join(ROOT, "profiles", "r2_traffic.json")
-        if os.path.exists(tp):
-            k = json.load(open(tp)).get(name, {}).get(dom)
-            if k:
-                traffic = k["dram_bytes_per_frame"] * F
         roofline = {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s",
-                    "frac": achieved / peak, "traffic": traffic, "peak_source": how,
+                    "frac": achieved / peak, "peak_source": how,
                     "algorithmic_bytes_per_launch": alg_bytes, "kernel_ms_per_launch": ms / n,
                     "kernel_share_of_chain": (ms / 2) / chain_ms,
                     "chain": {"ms_per_step": chain_ms, "achieved": alg_bytes / (chain_ms / 1e3) / 1e9,

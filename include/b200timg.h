@@ -1,4 +1,4 @@
-/* b200timg.h -- C ABI of the B200-native timg hot path.
+/* b200timg.h -- C ABI of the H100-native timg hot path.
  *
  * Drop-in boundary for hzeller/timg's per-pixel hot path (paths below are relative to
  * the reference tree):
@@ -14,7 +14,7 @@
  * row-major, tightly packed (src/framebuffer.h:26-61).  Colours passed as uint32_t are
  * the four rgba_t bytes in memory order: r | g<<8 | b<<16 | a<<24.
  *
- * Every entry point runs hand-written sm_100a CUDA kernels.  There is NO CPU fallback:
+ * Every entry point runs hand-written sm_90a CUDA kernels.  There is NO CPU fallback:
  * if no CUDA device is usable, b200timg_ctx_create fails with B200TIMG_ENODEV and nothing
  * else can be called.
  *

@@ -2,7 +2,7 @@
 // (timg_b200/csrc/adapters.h) and libb200timg.so into one binary and drives BOTH canvases/scalers
 // through the reference's own plugin surface (ImageScaler, TerminalCanvas, BufferedWriteSequencer),
 // comparing the bytes that reach the file descriptor.  This is the drop-in proof at the C++ level:
-// same calls a timg maintainer's build would make (INTEGRATION.md).  Needs a B200.
+// same calls a timg maintainer's build would make (INTEGRATION.md).  Needs a GPU.
 #include <fcntl.h>
 #include <sys/mman.h>
 #include <unistd.h>

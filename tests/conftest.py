@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a machine that has one)")
     if os.environ.get("B200TIMG_CUSIM"):      # developer aid: replay the GPU tests on tools/cusim (no GPU needed)
         from tools import cusim
         cusim.activate()

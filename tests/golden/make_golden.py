@@ -1,9 +1,9 @@
 """Regenerates tests/golden/*.npz from the reference itself (oracle/_ref/libtimg_ref.so, i.e. the
-UNMODIFIED timg translation units compiled by oracle/Makefile).  Run in the build container
-(where /root/reference exists):   python tests/golden/make_golden.py
+UNMODIFIED timg translation units compiled by oracle/Makefile, which needs the reference's sources):
+    python tests/golden/make_golden.py
 
 Inputs are not stored: tests/cases.py regenerates them deterministically.  Outputs are stored
-in full (zip-compressed), keyed by case name.
+in full (zip-compressed), keyed by case name, except the large ones of reference.npz (digests).
 """
 import os
 import sys
@@ -47,6 +47,41 @@ def main():
     np.savez_compressed(os.path.join(HERE, "fit.npz"), rows=np.array(fit, np.float64))
     total = sum(os.path.getsize(os.path.join(HERE, f)) for f in os.listdir(HERE) if f.endswith(".npz"))
     print(f"wrote {len(blocks)} block outputs, {len(comp)} compose outputs, {len(fit)} fit rows; {total} bytes")
+    reference()
+
+
+def reference():
+    """reference.npz: what the tests that once called the reference directly compare against.  Small outputs
+    are stored in full; frames and canvases of the config geometries as SHA-256 digests (cases.sha)."""
+    bg = oracle.rgba_u32(0, 0, 0)
+    g = {"as256": np.array([oracle.ref().ref_as256(v) for v in cases.as256_values()], np.uint8)}
+    for seed in range(6):
+        outs = cases.run_block_case(lambda *f: oracle.RefBlockCanvas(*f), cases.random_block_case(seed))
+        for i, o in enumerate(outs):
+            g[f"blocks_random/{seed}/{i}"] = np.frombuffer(o, np.uint8)
+    for i, (fb, kw) in enumerate(cases.random_compose_cases()):
+        g[f"compose_random/{i}"] = oracle.ref_compose_bg(fb, **kw)
+    for i, (img, ow, oh, fmt) in enumerate(cases.random_scale_cases()):
+        g[f"scale_random/{i}"] = cases.sha(oracle.ref_scale(img, ow, oh, fmt))
+    for iw, ih, fit, kind in cases.CONFIG_GEOMETRIES:
+        _, ow, oh = oracle.calc_fit(iw, ih, *fit)
+        s = oracle.ref_scale(cases.config_frame(iw, ih, kind), ow, oh)
+        g[f"config_scale/{iw}x{ih}-{ow}x{oh}"] = cases.sha(s)
+        g[f"config_compose/{iw}x{ih}-{ow}x{oh}"] = cases.sha(oracle.ref_compose_bg(s, bg))
+    for f, fr in enumerate(cases.c1_frames()):
+        fb = oracle.ref_compose_bg(oracle.ref_scale(fr, 67, 50), bg)
+        g[f"c1_blocks/{f}"] = cases.sha(oracle.RefBlockCanvas(False).send(fb))
+    cv = oracle.RefBlockCanvas(True)
+    for f, fr in enumerate(cases.c3_frames()):
+        fb = oracle.ref_compose_bg(oracle.ref_scale(fr, 320, 90), bg)
+        g[f"c3_blocks/{f}"] = cases.sha(cv.send(fb, 0, 0 if f == 0 else -90))
+    for f, fr in enumerate(cases.c4_frames()):
+        fb = np.zeros((192, 337, 4), np.uint8)                            # 337x190, padded to a multiple of 6 rows
+        fb[:190] = oracle.ref_compose_bg(oracle.ref_scale(fr, 337, 190), bg)
+        g[f"c4_padded/{f}"] = cases.sha(oracle.ref_compose_bg(fb, bg, start_row=190))
+    g = {k: np.frombuffer(v, np.uint8) if isinstance(v, bytes) else v for k, v in g.items()}
+    np.savez_compressed(os.path.join(HERE, "reference.npz"), **g)
+    print(f"wrote {len(g)} reference outputs; {os.path.getsize(os.path.join(HERE, 'reference.npz'))} bytes")
 
 
 if __name__ == "__main__":

@@ -3,8 +3,8 @@
 This module is harness plumbing for tests and bench.py: it loads the in-tree shared
 library with ctypes, declares every symbol of the ABI, and offers small numpy/torch
 conveniences.  The product is the CUDA library; there is no Python or CPU fallback:
-loading fails loudly if the library is missing, and Context() raises if no B200 is
-visible.
+loading fails loudly if the library is missing, and Context() raises if no CUDA
+device is visible.
 """
 import ctypes as C
 import os
@@ -103,7 +103,7 @@ _lib = None
 
 
 def build(verbose=False):
-    """Compile every CUDA source for sm_100a into timg_b200/libb200timg.so (in-tree)."""
+    """Compile every CUDA source for sm_90a into timg_b200/libb200timg.so (in-tree)."""
     subprocess.run(["make", "-C", os.path.join(_HERE, "csrc"), "-j8"], check=True,
                    stdout=None if verbose else subprocess.DEVNULL)
 

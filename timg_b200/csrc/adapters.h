@@ -59,7 +59,7 @@ private:
         const char *dev = getenv("TIMG_B200_DEVICE");
         const int rc = b200timg_ctx_create(dev ? atoi(dev) : 0, nullptr, &ctx_);
         if (rc != B200TIMG_OK) {   // no CPU fallback by design
-            fprintf(stderr, "b200timg: no usable B200 (error %d)\n", rc);
+            fprintf(stderr, "b200timg: no usable CUDA device (error %d)\n", rc);
             abort();
         }
     }

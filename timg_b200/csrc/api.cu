@@ -463,8 +463,8 @@ static int sixel_batch_phases(b200timg_ctx *ctx, const b200timg_batch *b, const 
     // latency-bound (one CTA per frame), so the scaler and the emitter of the other slices fill the machine meanwhile.
     // Timing runs (b200timg_profile) keep the plain in-order chain so that per-kernel durations stay meaningful.
     int parts = 1;
-    // measured (run r2k): 1250 unscaled 720p frames 29.9 -> 28.3 ms with 4 slices; 148 4K frames 14.28 vs 14.25 ms with 2 -- not
-    // worth a second launch sequence, so batches below 512 frames stay one in-order chain
+    // slices pay for thousands of small frames (C5); for a batch of some hundred 4K frames a second launch sequence
+    // gains nothing, so batches below 512 frames stay one in-order chain
     if (phases == 3 && !ctx->profiling && !ctx->ev_after_scale && b->n_frames >= 512) parts = 4;
     if (const char *e = getenv("B200TIMG_PARTS")) parts = std::max(1, std::min(4, std::min(atoi(e), b->n_frames)));
     if (parts == 1) {

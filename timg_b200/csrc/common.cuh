@@ -61,7 +61,7 @@ struct b200timg_ctx {
     int resident_w = 0, resident_h = 0;       // ... (cleared by anything else that writes fb_scaled)
     cudaStream_t stream = nullptr;
     bool own_stream = false;
-    int sm_count = 148;
+    int sm_count = 132;                       // H100 SXM; replaced by the device's count at ctx creation
     uint64_t launches = 0;
     char err[512] = {0};
     // optional per-kernel timing (b200timg_profile): CUDA events on the launching stream

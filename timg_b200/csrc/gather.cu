@@ -79,8 +79,8 @@ gather_offsets_kernel(unsigned long long *__restrict__ offs, int nranks, int n1,
 static int gather_streams(b200timg_ctx *ctx) {
     if (ctx->gather_stream) return B200TIMG_OK;
     // highest priority: the NCCL send/recv kernels must get SM slots WHILE the next batch's kernels run -- at equal priority the
-    // block scheduler keeps feeding the running compute grid and the transfer only advances in the gaps between kernels
-    // (4 GPUs: 15.4 ms per step against 13.1 on one; fewer NCCL channels made it worse, 17-18 ms: run r2n4)
+    // block scheduler keeps feeding the running compute grid and the transfer only advances in the gaps between kernels;
+    // fewer NCCL channels make that worse
     int prio_least = 0, prio_greatest = 0;
     B2_CUDA(ctx, cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest));
     B2_CUDA(ctx, cudaStreamCreateWithPriority(&ctx->gather_stream, cudaStreamNonBlocking, prio_greatest));

@@ -517,8 +517,8 @@ resample_fixed_kernel(const uint32_t *__restrict__ in, uint32_t *__restrict__ ou
 }
 
 // ---- planar fast path (vertical pass first, <= 8 taps per axis) ---------------------------
-// Same arithmetic again, reorganised around what limits resample_fixed_kernel on B200 (shared-memory
-// wavefronts and issue slots, see profiles/): every filtered channel is an independent plane, so the
+// Same arithmetic again, reorganised around what limits resample_fixed_kernel (shared-memory
+// wavefronts and issue slots): every filtered channel is an independent plane, so the
 // window is staged as separate float planes and
 //   * the vertical pass produces 4 neighbouring columns per thread (one LDS.128 per tap and plane),
 //   * the horizontal pass maps lanes to output ROWS: a warp works on one output column at a time, its
@@ -788,8 +788,8 @@ static PlanarFn planar_h(int hc, int vc) {
 
 typedef void (*FixedFn)(const uint32_t *, uint32_t *, ResampleParams, FixedGeom);
 struct FixedVariant { FixedFn fn; int th, nt; };
-// Tile 64x16, 256 threads, 3 CTAs/SM (80 registers) measured best on B200 among {16x256x3, 16x256x4,
-// 8x128x8, 8x256x4, 16x512x2, 32x512x2} (4.21 / 4.76 / 5.01 / 4.79 / 5.45 / 6.75 ms for 64 C2 frames).
+// Tile 64x16, 256 threads, 3 CTAs/SM (80 registers of the SM's 64 K), chosen among {16x256x3, 16x256x4,
+// 8x128x8, 8x256x4, 16x512x2, 32x512x2} for C2 frames.
 template <bool VF, int HC>
 static FixedVariant fixed_v(int vc, char v) {
     switch (vc) {
@@ -1050,13 +1050,12 @@ resample_copy4_kernel(const uint32_t *__restrict__ in, uint32_t *__restrict__ ou
 // sums: it stages three float planes (12 B/px) and every tap of the vertical pass is a 16-byte load.
 // v3 keeps the window as the RAW pixels (4 B/px: a plain 16-byte copy, no decode at staging) and turns
 // bytes into floats at the point of use (PRMT into the mantissa of 2^23, one FSUB), two neighbouring
-// columns per thread; the tap sums work on register PAIRS -- (R,G) of a pixel, (B,B) of two pixels --
-// so one packed instruction does two channels.  Two arithmetic modes:
+// columns per thread; the tap sums work on register PAIRS -- (R,G) of a pixel, (B,B) of two pixels.
+// Two arithmetic modes:
 //   EXACT  the reference's arithmetic bit for bit (byte * (1/255), every product and sum rounded
-//          separately: scalar FMUL + packed FADD2 -- ptxas contracts mul.f32x2 + add.f32x2 into FFMA2 no
-//          matter what, so the products stay scalar), even/odd horizontal accumulators, analytic alpha
+//          separately: FMUL + FADD, never contracted), even/odd horizontal accumulators, analytic alpha
 //          of the all-opaque window, un-weight by 1/alpha, trunc(clamp(v * 255 + 0.5));
-//   FAST   the same filter with FFMA2 and the 1/255 .. *255 round trip dropped: within 1 LSB of the
+//   FAST   the same filter with FFMA and the 1/255 .. *255 round trip dropped: within 1 LSB of the
 //          reference (BASELINE.md's stated gate for the Mitchell path); used where the result feeds the
 //          sixel quantiser, whose own parity is a delta-E tolerance.
 // Tiles whose window is not fully opaque are handed to the planar kernel through a work list.
@@ -1065,14 +1064,10 @@ struct F2 { float x, y; };
 __device__ __forceinline__ F2 f2_add(F2 a, F2 b) { return F2{a.x + b.x, a.y + b.y}; }
 __device__ __forceinline__ F2 f2_fma(F2 a, F2 b, F2 c) { return F2{fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)}; }
 #else
-__device__ __forceinline__ unsigned long long f2_pack(F2 a) { unsigned long long r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a.x), "f"(a.y)); return r; }
-__device__ __forceinline__ F2 f2_unpack(unsigned long long v) { F2 r; asm("mov.b64 {%0, %1}, %2;" : "=f"(r.x), "=f"(r.y) : "l"(v)); return r; }
-__device__ __forceinline__ F2 f2_add(F2 a, F2 b) {
-    unsigned long long r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(f2_pack(a)), "l"(f2_pack(b))); return f2_unpack(r);
-}
-__device__ __forceinline__ F2 f2_fma(F2 a, F2 b, F2 c) {
-    unsigned long long r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(f2_pack(a)), "l"(f2_pack(b)), "l"(f2_pack(c))); return f2_unpack(r);
-}
+// sm_90 has no packed FP32 arithmetic: each lane is one round-to-nearest FADD / FFMA (__fadd_rn is never
+// contracted with the product before it, which the EXACT mode relies on).
+__device__ __forceinline__ F2 f2_add(F2 a, F2 b) { return F2{__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)}; }
+__device__ __forceinline__ F2 f2_fma(F2 a, F2 b, F2 c) { return F2{__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)}; }
 #endif
 // acc = v * c   /   acc += v * c   in the mode's arithmetic
 template <bool EXACT> __device__ __forceinline__ F2 f2_mul(F2 v, float c) {
@@ -1111,18 +1106,18 @@ __device__ __forceinline__ uint32_t sat_u8(float v) {
 }
 
 struct V3Geom { int nix, niy, sp, tp; unsigned grp_magic; const int32_t *tile_ix0, *tile_iy0; uint32_t *fallback; int use_tma; };   // grp_magic: floor(2^32/(sp/4))+1
-// Tuning switches (tools/build_variant.sh builds variant libraries; measured per 148 C2 frames, run r2k):
-//   V3_SENT 0, 2 CTAs/SM asked (78 registers, 3 resident anyway)   4.70 ms   <- default
-//   V3_SENT 1, 3 CTAs/SM forced (72 registers, more instructions)  5.36 ms
-//   V3_SENT 1, 2 CTAs/SM (84 registers: only 2 resident)           6.05 ms
-//   V3_SENT 0, 3 CTAs/SM forced (80 registers, spills)             6.03 ms
+// Tuning switches (tools/build_variant.sh builds variant libraries to compare on C2 frames):
+//   V3_SENT 0, 2 CTAs/SM asked (3 resident when it fits 80 registers)   <- default
+//   V3_SENT 1, 3 CTAs/SM forced (fewer registers, more instructions)
+//   V3_SENT 1, 2 CTAs/SM (more than 80 registers: only 2 resident)
+//   V3_SENT 0, 3 CTAs/SM forced (80 registers, spills)
 #ifndef V3_SENT
 #define V3_SENT 0            // 1: sentinel-terminated completion walks (no bound test), 0: bounded walks
 #endif
 #ifndef V3_MINB_VALUE
 #define V3_MINB_VALUE 2
 #endif
-constexpr int V3_TW = 64, V3_TH = 32, V3_NT = 256, V3_MINB = V3_MINB_VALUE;   // 3 CTAs/SM: <= 80 registers (84 cost a third of the occupancy: 5.06 -> 6.05 ms)
+constexpr int V3_TW = 64, V3_TH = 32, V3_NT = 256, V3_MINB = V3_MINB_VALUE;   // 3 CTAs/SM: <= 80 registers (84 cost a third of the occupancy)
 
 template <int HC, int VC, bool EXACT>
 __global__ void __launch_bounds__(V3_NT, (VC >= 8 ? 2 : V3_MINB))      // the 8-row register windows do not fit 80 registers
@@ -1509,7 +1504,7 @@ int launch_scale(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int fmt
             const int ntx = (int)tix.size(), nty = (int)tiy.size();
             const int sp = (nix + 3) & ~3, tp = sp | 1;   // odd T pitch >= the 4-column groups written per row
             const size_t psmem = sizeof(float) * (3 * ((size_t)niy * sp + (size_t)PTH * tp) + 4 + (size_t)ptw * 8 + PTH * 8) + sizeof(int) * (ptw + PTH);
-            const size_t smem_cap = 75 * 1024;           // 3 CTAs/SM (80 registers): 7.96 ms vs 10.2 ms at 2 CTAs/SM, 148 C2 frames
+            const size_t smem_cap = 75 * 1024;           // 3 CTAs/SM (80 registers) rather than 2
             const bool planar_ok = psmem <= smem_cap && (size_t)PTH * (ptw + 1) <= 3 * (size_t)niy * sp;
             // v3 geometry: 64 x 32 output tiles
             const int nix3 = tile_origins(pl->h, ow, V3_TW, hc, true, tix3);
@@ -1517,8 +1512,8 @@ int launch_scale(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int fmt
             const int sp3 = (nix3 + 3) & ~3, tp3 = sp3 | 1;
             const size_t v3smem = sizeof(uint32_t) * (size_t)niy * sp3 + (sizeof(float2) + sizeof(float)) * (size_t)V3_TH * tp3 + 16 +
                                   sizeof(float) * ((size_t)V3_TW * 8 + V3_TH * 8) + sizeof(int) * (V3_TW + V3_TH + 2);
-            // v3 pays off in the FAST arithmetic (5.4 vs 7.9 ms per 148 C2 frames); in EXACT arithmetic its streaming passes are
-            // slower than the planar kernel (9.3 vs 7.9 ms), so bit-exact scaling stays on the planar kernel unless asked
+            // v3 pays off in the FAST arithmetic; in EXACT arithmetic its streaming passes are slower than the planar
+            // kernel, so bit-exact scaling stays on the planar kernel unless asked
             const bool v3_ok = planar_ok && !getenv("B200TIMG_NO_V3") && (fast || getenv("B200TIMG_V3_EXACT")) && v3smem <= 100 * 1024 &&
                                (size_t)V3_TH * (V3_TW + 1) <= (size_t)niy * sp3;
             if (planar_ok) {
@@ -1625,8 +1620,8 @@ int launch_scale(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int fmt
                     }
                     const size_t h1smem = sizeof(float4) * 8 * (size_t)HG.nwin + sizeof(float) * 32 * (size_t)HG.cpitch;
                     B2_KERNEL(ctx, plain ? "twopass_plain_kernels" : "twopass_h1_kernel");
-                    // staging pays when the 32-column tiles are mostly full (4K -> 337 columns: 6.53 -> 5.42 ms per 128 frames); with
-                    // 67 columns the third tile stages a whole window for 3 outputs (8.23 -> 8.73 ms per 4096 frames): plain kernel
+                    // staging pays when the 32-column tiles are mostly full (4K -> 337 columns); with 67 columns the third
+                    // tile stages a whole window for 3 outputs: plain kernel
                     const bool tiles_full = (long long)((ow + 31) / 32) * 32 * 100 <= (long long)ow * 115;
                     if (h1smem <= 72 * 1024 && tiles_full && !getenv("B200TIMG_NO_H1S")) {
                         if (plain) {

@@ -711,7 +711,7 @@ sixel_emit_kernel(EmitGeom G, SixelWork W) {
 }
 
 // ---- emit v1b: one walk instead of two -------------------------------------------------------------------------------
-// profiles/r2_lines_sixel_emit_v1.txt: v1 spends ~21 % of its instructions in the sizes walk and ~31 % in the byte-wise,
+// Per-line instruction counts show v1 spending a large share of its instructions in the sizes walk and in the byte-wise,
 // heavily divergent formatting of the write walk (every lane of a warp sits in another branch of put_rle / put_num4 and
 // stores single bytes to global memory).  v1b walks the sorted entries ONCE: every run head builds its <= 3 pieces
 // (colour introducer, gap, run) as 64-bit values with branch-light arithmetic and appends them to a thread-private slot
@@ -1055,8 +1055,7 @@ static int sixel_plan(b200timg_ctx *ctx, int w, int h, int n_frames, bool reserv
     const size_t o_scr = off;
     // three emitters (B200TIMG_EMIT=1|2|3): v1 (the default up to 4095 px: per-band sizes into a scratch arena + compaction
     // kernel), emit2 (sixel_emit.cu: single pass, any width -- what wider frames get) and emit3 (v1's sort + entry-parallel
-    // formatting + look-back placement; measured SLOWER than v1, profiles/r2_notes.md: 9.2 ms without and 63 ms with the
-    // look-back against v1's 5.2 + 0.36 ms per 148 C2 frames; kept for A/B runs only).
+    // formatting + look-back placement; slower than v1 on C2 frames, kept for A/B runs only).
     {
         const bool v1_fits = w <= 4095 && sizeof(uint32_t) * (size_t)6 * w <= (size_t)(227 - 36) * 1024;
         const bool v1b_fits = w <= 4095 && sizeof(uint32_t) * (size_t)6 * w <= (size_t)(227 - 47) * 1024;

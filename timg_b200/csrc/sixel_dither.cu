@@ -259,8 +259,8 @@ size_t sixel_dither_workspace(int w, int h, int n_frames, size_t *o_bnd, size_t 
 int launch_sixel_dither(b200timg_ctx *ctx, const uint32_t *fb, int w, int h, int n_frames, int n_total, const SixelWork &W, void *d_bnd, void *d_prog) {
     Dither2Geom G;
     G.w = w; G.h = h; G.nb32 = (h + 31) / 32;
-    // A chunk of 16 columns x 32 rows takes a warp several microseconds; polling the band above every 32 ns spent 13.6 % of
-    // the kernel's issue slots in the wait loop (profiles/r2_lines_sixel_dither2.txt), slots the producing warps need.
+    // A chunk of 16 columns x 32 rows takes a warp several microseconds; polling the band above every 32 ns spends a
+    // noticeable share of the kernel's issue slots in the wait loop, slots the producing warps need.
     G.spin_ns = 256;
     if (const char *e = getenv("B200TIMG_DITHER_SPIN")) G.spin_ns = (unsigned)std::max(0, std::min(atoi(e), 100000));
     // CTAs per frame: 1 when the batch fills the GPU, more (up to one round of bands per CTA) for small batches.

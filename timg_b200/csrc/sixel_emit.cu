@@ -316,14 +316,14 @@ sixel_header_kernel(int w, int h, SixelWork W) {
 
 
 // ---------------------------------------------------------------------------------------------------------
-// emit3 (EXPERIMENT, B200TIMG_EMIT=3; not the default: it measured slower than v1, see profiles/r2_notes.md).  Same
+// emit3 (EXPERIMENT, B200TIMG_EMIT=3; not the default: it is slower than v1).  Same
 // grammar and the same bytes as the two-pass v1 emitter of sixel.cu, built from
 //   * v1's per-band counting sort (warps own column ranges, per-warp count / mask tables),
 //   * an ENTRY-PARALLEL sizing and formatting stage: a warp takes 32 consecutive sorted entries at a time; run heads,
 //     run lengths (next head in the ballot), gaps and byte sizes are lane-local arithmetic on the neighbouring
 //     entries, offsets are a warp scan, and every head writes its <= 3 pieces (colour introducer, gap, run) into a
 //     shared-memory window -- v1 walked ~16 entries per THREAD with data-dependent loops and single-byte global
-//     stores (profiles/r2_lines_sixel_emit_v1.txt: two thirds of its 104 K warp-instructions per band),
+//     stores (most of its warp-instructions per band),
 //   * emit2's placement: ticketed CTAs, decoupled look-back over per-CTA byte counts, the window copied to its final
 //     place with aligned word stores.  No per-band scratch arena, no compaction kernel.
 constexpr int E3T = 512, E3W = E3T / 32;

@@ -1,5 +1,5 @@
 """Multi-GPU plumbing for the frame-sharded path (SURVEY.md 8e): frames are independent units,
-each rank encodes a contiguous chunk on its own B200, and the only exchange is the gather of the
+each rank encodes a contiguous chunk on its own GPU, and the only exchange is the gather of the
 encoded byte buffers to rank 0 (NCCL on GPUs; the same code runs over gloo on CPU for tests).
 
 The reference has no counterpart (single process; frames go one Send() at a time to one tty,

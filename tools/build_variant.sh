@@ -4,8 +4,8 @@
 set -e
 cd "$(dirname "$0")/../timg_b200/csrc"
 tag=$1; shift
-NV="/usr/local/cuda/bin/nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -fmad=false -Xcompiler -fPIC,-ffp-contract=off -I../../include"
+NV="/usr/local/cuda/bin/nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -fmad=false -Xcompiler -fPIC,-ffp-contract=off -I../../include"
 $NV "$@" -c resample.cu -o /tmp/resample_$tag.o -Xptxas -v 2> /tmp/resample_$tag.log
 objs=$(ls *.o | grep -v '^resample\.o$' | tr '\n' ' ')
-/usr/local/cuda/bin/nvcc -gencode arch=compute_100a,code=sm_100a -shared -o ../libb200timg_$tag.so $objs /tmp/resample_$tag.o -cudart static
+/usr/local/cuda/bin/nvcc -gencode arch=compute_90a,code=sm_90a -shared -o ../libb200timg_$tag.so $objs /tmp/resample_$tag.o -cudart static
 grep -A2 "resample_v3_kernelILi6ELi6ELb0" /tmp/resample_$tag.log | grep -E "Used|spill" 

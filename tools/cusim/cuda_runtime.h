@@ -74,7 +74,7 @@ static inline cudaError_t cudaGetLastError() { return cudaSuccess; }
 static inline cudaError_t cudaPeekAtLastError() { return cudaSuccess; }
 static inline const char *cudaGetErrorString(cudaError_t) { return "cusim"; }
 static inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int) {
-    memset(p, 0, sizeof *p); strcpy(p->name, "cusim"); p->multiProcessorCount = 148; p->major = 10; p->minor = 0;
+    memset(p, 0, sizeof *p); strcpy(p->name, "cusim"); p->multiProcessorCount = 132; p->major = 9; p->minor = 0;
     return cudaSuccess;
 }
 static inline cudaError_t cudaMalloc(void **p, size_t n) { *p = aligned_alloc(256, (n + 255) / 256 * 256 + 256); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
