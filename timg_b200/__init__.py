@@ -18,6 +18,7 @@ LIB_PATH = os.environ.get("B200TIMG_LIBFILE") or os.path.join(_HERE, "libb200tim
 OK, EINVAL, ENOMEM, ECUDA, ENOSPC, ENODEV = 0, -1, -2, -3, -4, -5
 QUARTER, UPPER, COLOR8, FAST_SCALE, BILINEAR_SCALE = 1, 2, 4, 8, 16
 FMT_RGBA, FMT_RGB32, FMT_I420, FMT_NV12, FMT_FULL_RANGE = 0, 1, 2, 3, 0x10
+KITTY, ITERM2 = 1, 2
 
 u8p = C.POINTER(C.c_uint8)
 u64p = C.POINTER(C.c_uint64)
@@ -34,6 +35,10 @@ class Batch(C.Structure):
                 ("out_w", C.c_int), ("out_h", C.c_int), ("has_bg", C.c_int), ("bg", C.c_uint32),
                 ("pattern", C.c_uint32), ("pattern_w", C.c_int), ("pattern_h", C.c_int),
                 ("flags", C.c_int), ("x_indent_cells", C.c_int), ("animation", C.c_int)]
+
+
+class Graphics(C.Structure):
+    _fields_ = [("protocol", C.c_int), ("rgb24", C.c_int), ("ids", C.POINTER(C.c_uint32))]
 
 
 # name -> (restype, argtypes); this table IS the list of exported symbols tests check.
@@ -85,6 +90,11 @@ ABI = {
     "b200timg_base64_size": (C.c_size_t, [C.c_size_t]),
     "b200timg_png_encode": (C.c_int, [C.c_void_p, u8p, C.c_int, C.c_int, C.c_int, u8p, C.c_size_t, C.c_char_p, C.c_size_t]),
     "b200timg_png_batch_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "b200timg_graphics_size": (C.c_size_t, [C.POINTER(Graphics), C.c_int, C.c_int, C.c_uint32]),
+    "b200timg_graphics_batch_dev": (C.c_int, [C.c_void_p, C.POINTER(Batch), C.POINTER(Graphics), C.c_void_p, C.c_void_p,
+                                              C.c_size_t, C.c_void_p]),
+    "b200timg_graphics_batch": (C.c_int, [C.c_void_p, C.POINTER(Batch), C.POINTER(Graphics), C.c_void_p, C.c_void_p,
+                                          C.c_size_t, C.c_void_p]),
     "b200timg_gather_unique_id": (C.c_int, [C.c_char_p]),
     "b200timg_gather_init": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int, C.c_int]),
     "b200timg_gather_attach": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
@@ -160,6 +170,19 @@ def resample_plan(iw, ih, ow, oh, axis):
         raise B200Error(rc, "resample_plan")
     return dict(widest=widest.value, flags=flags.value, first=first, count=count, lead=lead,
                 coeff=coeff.reshape(n, widest.value))
+
+
+def graphics(protocol, rgb24=False, ids=None):
+    """(b200timg_graphics, the uint32 id array it points to): keep both alive for the call."""
+    arr = None if ids is None else np.ascontiguousarray(ids, dtype=np.uint32)
+    g = Graphics(protocol, int(rgb24), arr.ctypes.data_as(C.POINTER(C.c_uint32)) if arr is not None else None)
+    return g, arr
+
+
+def graphics_size(protocol, w, h, rgb24=False, id=0):
+    """Exact bytes of one framed kitty / iTerm2 frame (host only)."""
+    g, _ = graphics(protocol, rgb24)
+    return lib().b200timg_graphics_size(C.byref(g), w, h, id)
 
 
 def _np_ptr(a):
@@ -325,3 +348,37 @@ class Context:
 
     def sixel_batch(self, frames, b):
         return self._batch_host(lib().b200timg_sixel_batch, frames, b, sixel=True)
+
+    def graphics_batch(self, frames, b, protocol, rgb24=False, ids=None, with_offsets=False):
+        """Framed kitty / iTerm2 text of every frame (list of bytes); ids: one kitty image id per frame.
+        frames: numpy source frames (RGBA [n,h,w,4], or flat YUV bytes per frame)."""
+        frames = np.ascontiguousarray(frames, dtype=np.uint8)
+        n = b.n_frames
+        g, keep = graphics(protocol, rgb24, ids)
+        sizes = [lib().b200timg_graphics_size(C.byref(g), b.out_w, b.out_h, int(keep[f]) if keep is not None else 0)
+                 for f in range(n)]
+        cap = max(1, sum(sizes))
+        out = np.empty(cap, np.uint8)
+        offs = np.zeros(n + 1, np.uint64)
+        self._chk(lib().b200timg_graphics_batch(self.h, C.byref(b), C.byref(g), frames.ctypes.data, out.ctypes.data, cap,
+                                                offs.ctypes.data))
+        res = [out[int(offs[i]):int(offs[i + 1])].tobytes() for i in range(n)]
+        return (res, offs) if with_offsets else res
+
+    def graphics_batch_dev(self, d_src, b, protocol, rgb24=False, ids=None, d_out=None, out_cap=None, d_offsets=None):
+        """Device-resident variant on torch CUDA tensors: returns (d_out, d_offsets) after the (asynchronous) call;
+        allocates them when not given (out_cap defaults to the exact size of the batch)."""
+        import torch
+        g, keep = graphics(protocol, rgb24, ids)
+        n = b.n_frames
+        if d_out is None:
+            need = sum(lib().b200timg_graphics_size(C.byref(g), b.out_w, b.out_h, int(keep[f]) if keep is not None else 0)
+                       for f in range(n))
+            d_out = torch.empty(max(1, need), dtype=torch.uint8, device=d_src.device)
+        if out_cap is None:
+            out_cap = d_out.numel()
+        if d_offsets is None:
+            d_offsets = torch.empty(n + 1, dtype=torch.int64, device=d_src.device)
+        self._chk(lib().b200timg_graphics_batch_dev(self.h, C.byref(b), C.byref(g), d_src.data_ptr(), d_out.data_ptr(),
+                                                    out_cap, d_offsets.data_ptr()))
+        return d_out, d_offsets

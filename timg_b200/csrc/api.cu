@@ -75,6 +75,8 @@ void b200timg_ctx_destroy(b200timg_ctx *ctx) {
     ctx->out_stage.release(); ctx->offsets.release(); ctx->cells.release(); ctx->rows.release();
     ctx->tables.release(); ctx->sixel_work.release(); ctx->misc.release(); ctx->scale_list.release(); ctx->scale_tmp.release(); ctx->tri_tables.release();
     ctx->pinned.release(); ctx->pinned_io.release();
+    ctx->png_sums.release(); ctx->gfx_ids.release();
+    for (int i = 0; i < 4; ++i) { ctx->gfx_stage[i].release(); if (ctx->ev_gfx[i]) cudaEventDestroy(ctx->ev_gfx[i]); }
     for (int i = 0; i < 2; ++i) { ctx->pipe_in[i].release(); ctx->pipe_out[i].release(); }
     if (ctx->parts_ready) {
         for (int i = 0; i < 4; ++i) { cudaStreamSynchronize(ctx->part_stream[i]); cudaStreamDestroy(ctx->part_stream[i]); cudaEventDestroy(ctx->ev_part[i]); }
@@ -505,6 +507,59 @@ int b200timg_sixel_batch_dev(b200timg_ctx *ctx, const b200timg_batch *b, const u
     return sixel_batch_phases(ctx, b, d_src, d_out, out_cap, d_offsets, 3);
 }
 
+// ---- kitty / iTerm2 batches ------------------------------------------------------------------
+static int validate_graphics(b200timg_ctx *ctx, const b200timg_batch *b, const b200timg_graphics *g) {
+    if (!g) return ctx->fail(B200TIMG_EINVAL, "graphics: null protocol description");
+    if (g->protocol != B200TIMG_KITTY && g->protocol != B200TIMG_ITERM2) return ctx->fail(B200TIMG_EINVAL, "graphics: unknown protocol %d", g->protocol);
+    if (g->protocol == B200TIMG_KITTY && !g->ids) return ctx->fail(B200TIMG_EINVAL, "graphics: kitty needs one image id per frame (ids is NULL)");
+    if (b->animation != 0) return ctx->fail(B200TIMG_EINVAL, "graphics: kitty / iTerm2 frames have no delta encoding (animation must be 0)");
+    if (b200timg_png_size(b->out_w, b->out_h, g->rgb24) > 0x7fffffffu)
+        return ctx->fail(B200TIMG_EINVAL, "graphics: the PNG of a %dx%d frame does not fit one IDAT chunk", b->out_w, b->out_h);
+    return B200TIMG_OK;
+}
+
+// offsets[0..n]: the running sum of the frame sizes
+static void graphics_offsets(const b200timg_batch *b, const b200timg_graphics *g, uint64_t *offsets) {
+    offsets[0] = 0;
+    const bool kitty = g->protocol == B200TIMG_KITTY;
+    for (int f = 0; f < b->n_frames; ++f) offsets[f + 1] = offsets[f] + b200timg_graphics_size(g, b->out_w, b->out_h, kitty ? g->ids[f] : 0);
+}
+
+int b200timg_graphics_batch_dev(b200timg_ctx *ctx, const b200timg_batch *b, const b200timg_graphics *g,
+                                const uint8_t *d_src, char *d_out, size_t out_cap, uint64_t *d_offsets) {
+    B2_TRY(check_ctx(ctx));
+    B2_TRY(validate_batch(ctx, b));
+    if (!d_src || !d_out || !d_offsets) return ctx->fail(B200TIMG_EINVAL, "batch: null pointer");
+    B2_TRY(validate_graphics(ctx, b, g));
+    const int n = b->n_frames;
+    const bool kitty = g->protocol == B200TIMG_KITTY;
+    // offsets (and kitty's ids) are computed here and go up from a pinned slot; the slot is only rewritten once the
+    // copy that last read it has run, which never waits unless four batches are queued behind each other
+    const int slot = ctx->gfx_slot;
+    ctx->gfx_slot = (slot + 1) % 4;
+    if (ctx->ev_gfx[slot]) B2_CUDA(ctx, cudaEventSynchronize(ctx->ev_gfx[slot]));
+    else B2_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_gfx[slot], cudaEventDisableTiming));
+    const size_t off_bytes = (size_t)(n + 1) * sizeof(uint64_t), id_bytes = kitty ? (size_t)n * sizeof(uint32_t) : 0;
+    B2_CUDA(ctx, ctx->gfx_stage[slot].reserve(off_bytes + id_bytes));
+    uint64_t *h_offs = ctx->gfx_stage[slot].as<uint64_t>();
+    graphics_offsets(b, g, h_offs);
+    B2_CUDA(ctx, cudaMemcpyAsync(d_offsets, h_offs, off_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    if (kitty) {
+        B2_CUDA(ctx, ctx->gfx_ids.reserve(id_bytes));
+        memcpy(h_offs + n + 1, g->ids, id_bytes);
+        B2_CUDA(ctx, cudaMemcpyAsync(ctx->gfx_ids.p, h_offs + n + 1, id_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    }
+    B2_CUDA(ctx, cudaEventRecord(ctx->ev_gfx[slot], ctx->stream));
+    const size_t fb_bytes = (size_t)b->out_w * b->out_h * 4 * n;
+    ctx->resident_fb = nullptr;
+    B2_CUDA(ctx, ctx->fb_scaled.reserve(fb_bytes));
+    uint8_t *d_fb = ctx->fb_scaled.as<uint8_t>();
+    const ComposeSpec cs = make_compose_spec(b->has_bg, b->bg, b->pattern, b->pattern_w, b->pattern_h);
+    B2_TRY(batch_scale(ctx, b, d_src, d_fb, b->out_h, &cs));
+    if (ctx->ev_after_scale) B2_CUDA(ctx, cudaEventRecord(ctx->ev_after_scale, ctx->stream));
+    return launch_graphics(ctx, d_fb, b->out_w, b->out_h, n, g->rgb24, g->protocol, ctx->gfx_ids.as<uint32_t>(), d_offsets, d_out, out_cap);
+}
+
 static int pipe_init(b200timg_ctx *ctx) {
     if (ctx->pipe_ready) return B200TIMG_OK;
     B2_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
@@ -522,13 +577,15 @@ static int pipe_init(b200timg_ctx *ctx) {
 
 // Host-buffer batch: the batch is cut into chunks; while chunk k runs its kernels, chunk k+1 is
 // uploading and chunk k-1's encoded bytes are downloading (three streams, double-buffered staging).
-// Per chunk the encoded size is known before anything is written (sixel) or bounded (blocks), so
-// the caller's buffer is never overrun and *exactly* the encoded bytes cross PCIe on the way back.
+// Per chunk the encoded size is known before anything is written (sixel), bounded (blocks) or a closed
+// formula known before the call (graphics), so the caller's buffer is never overrun and *exactly* the
+// encoded bytes cross PCIe on the way back.
+enum class Encoder { blocks, sixel, graphics };
 static int batch_host_impl(b200timg_ctx *ctx, const b200timg_batch *b, const uint8_t *src, char *out,
-                           size_t out_cap, uint64_t *offsets, bool sixel);
+                           size_t out_cap, uint64_t *offsets, Encoder enc, const b200timg_graphics *gfx);
 static int batch_host(b200timg_ctx *ctx, const b200timg_batch *b, const uint8_t *src, char *out,
-                      size_t out_cap, uint64_t *offsets, bool sixel) {
-    const int rc = batch_host_impl(ctx, b, src, out, out_cap, offsets, sixel);
+                      size_t out_cap, uint64_t *offsets, Encoder enc, const b200timg_graphics *gfx = nullptr) {
+    const int rc = batch_host_impl(ctx, b, src, out, out_cap, offsets, enc, gfx);
     if (rc != B200TIMG_OK && ctx && ctx->pipe_ready) {      // nothing may still be reading or writing the caller's buffers
         cudaStreamSynchronize(ctx->copy_stream); cudaStreamSynchronize(ctx->stream); cudaStreamSynchronize(ctx->d2h_stream);
         cudaGetLastError();
@@ -536,21 +593,29 @@ static int batch_host(b200timg_ctx *ctx, const b200timg_batch *b, const uint8_t 
     return rc;
 }
 static int batch_host_impl(b200timg_ctx *ctx, const b200timg_batch *b, const uint8_t *src, char *out,
-                           size_t out_cap, uint64_t *offsets, bool sixel) {
+                           size_t out_cap, uint64_t *offsets, Encoder enc, const b200timg_graphics *gfx) {
     B2_TRY(check_ctx(ctx));
     B2_TRY(validate_batch(ctx, b));
     if (!src || !out || !offsets) return ctx->fail(B200TIMG_EINVAL, "batch: null pointer");
+    const bool sixel = enc == Encoder::sixel, graphics = enc == Encoder::graphics;
+    if (graphics) {                                            // every size is known now: nothing runs if they do not fit
+        B2_TRY(validate_graphics(ctx, b, gfx));
+        graphics_offsets(b, gfx, offsets);
+        if (offsets[b->n_frames] > out_cap)
+            return ctx->fail(B200TIMG_ENOSPC, "batch: need %llu bytes (have %zu)", (unsigned long long)offsets[b->n_frames], out_cap);
+    }
     B2_TRY(pipe_init(ctx));
     const size_t frame_bytes = src_frame_bytes(b);
     int chunk = (int)std::max<size_t>(1, ((size_t)672 << 20) / frame_bytes);
     if (const char *e = getenv("B200TIMG_CHUNK_FRAMES")) chunk = std::max(1, atoi(e));      // test knob
     // delta-encoded animations chain frame to frame: every chunk after the first re-uploads its predecessor's last
     // frame as a halo (animation = 2: scaled, used as the reference of the chunk's first frame, not emitted)
-    const bool anim = !sixel && b->animation != 0;
+    const bool anim = enc == Encoder::blocks && b->animation != 0;
     chunk = std::min(chunk, b->n_frames);
     const int n_chunks = (b->n_frames + chunk - 1) / chunk;
-    const size_t blocks_bound = sixel ? b200timg_sixel_bound(b->out_w, round_to_sixel(b->out_h)) * (size_t)chunk
-                                      : b200timg_blocks_bound(b->out_w, b->out_h) * (size_t)chunk + 64;
+    const size_t blocks_bound = sixel      ? b200timg_sixel_bound(b->out_w, round_to_sixel(b->out_h)) * (size_t)chunk
+                                : graphics ? b200timg_graphics_size(gfx, b->out_w, b->out_h, 0xffffffffu) * (size_t)chunk
+                                           : b200timg_blocks_bound(b->out_w, b->out_h) * (size_t)chunk + 64;
     for (int i = 0; i < 2 && i < n_chunks; ++i) B2_CUDA(ctx, ctx->pipe_in[i].reserve(frame_bytes * (chunk + 1)));
     B2_CUDA(ctx, ctx->offsets.reserve((size_t)(chunk + 2) * sizeof(uint64_t)));
     B2_CUDA(ctx, ctx->pinned.reserve((size_t)(chunk + 2) * sizeof(uint64_t)));
@@ -567,7 +632,7 @@ static int batch_host_impl(b200timg_ctx *ctx, const b200timg_batch *b, const uin
     B2_TRY(upload_chunk(0));
     if (n_chunks > 1) B2_TRY(upload_chunk(1));
     size_t base_bytes = 0;
-    offsets[0] = 0;
+    if (!graphics) offsets[0] = 0;
     for (int k = 0; k < n_chunks; ++k) {
         const int i = k & 1, f0 = k * chunk, nf = std::min(chunk, b->n_frames - f0);
         const int halo = (anim && k > 0) ? 1 : 0;             // the sub-batch then starts one frame early
@@ -579,20 +644,28 @@ static int batch_host_impl(b200timg_ctx *ctx, const b200timg_batch *b, const uin
         if (k >= 2) B2_CUDA(ctx, cudaEventSynchronize(ctx->ev_d2h[i]));            // pipe_out[i] is free again
         B2_CUDA(ctx, ctx->pipe_out[i].reserve(blocks_bound));
         ctx->ev_after_scale = ctx->ev_scaled[i];                                   // recorded once pipe_in[i] has been consumed
+        b200timg_graphics sub_gfx = {};
+        if (graphics) { sub_gfx = *gfx; if (gfx->ids) sub_gfx.ids = gfx->ids + f0; }
         const int rc_k = sixel ? sixel_batch_phases(ctx, &sub, d_in, ctx->pipe_out[i].as<char>(), blocks_bound, ctx->offsets.as<uint64_t>(), 3)
-                               : b200timg_blocks_batch_dev(ctx, &sub, d_in, ctx->pipe_out[i].as<char>(), blocks_bound,
-                                                           ctx->offsets.as<uint64_t>());
+                       : graphics ? b200timg_graphics_batch_dev(ctx, &sub, &sub_gfx, d_in, ctx->pipe_out[i].as<char>(), blocks_bound,
+                                                                ctx->offsets.as<uint64_t>())
+                                  : b200timg_blocks_batch_dev(ctx, &sub, d_in, ctx->pipe_out[i].as<char>(), blocks_bound,
+                                                              ctx->offsets.as<uint64_t>());
         ctx->ev_after_scale = nullptr;
         B2_TRY(rc_k);
         if (k + 2 < n_chunks) {                                                    // refill pipe_in[i] as soon as this chunk's scaler is done
             B2_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_scaled[i], 0));
             B2_TRY(upload_chunk(k + 2));
         }
-        B2_CUDA(ctx, cudaMemcpyAsync(h_offs, ctx->offsets.p, (size_t)(nf + halo + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
-        B2_CUDA(ctx, cudaEventRecord(ctx->ev_prep, ctx->stream));
-        B2_CUDA(ctx, cudaEventSynchronize(ctx->ev_prep));                          // sizes of this chunk are on the host
-        const size_t total = (size_t)h_offs[nf + halo];                            // a halo frame contributes no bytes
-        for (int j = 1; j <= nf; ++j) offsets[f0 + j] = base_bytes + h_offs[j + halo];
+        size_t total = 0;
+        if (graphics) total = (size_t)(offsets[f0 + nf] - offsets[f0]);           // known before the call
+        else {
+            B2_CUDA(ctx, cudaMemcpyAsync(h_offs, ctx->offsets.p, (size_t)(nf + halo + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
+            B2_CUDA(ctx, cudaEventRecord(ctx->ev_prep, ctx->stream));
+            B2_CUDA(ctx, cudaEventSynchronize(ctx->ev_prep));                      // sizes of this chunk are on the host
+            total = (size_t)h_offs[nf + halo];                                     // a halo frame contributes no bytes
+            for (int j = 1; j <= nf; ++j) offsets[f0 + j] = base_bytes + h_offs[j + halo];
+        }
         if (base_bytes + total > out_cap) {
             return ctx->fail(B200TIMG_ENOSPC, "batch: need more than %zu bytes (have %zu)", base_bytes + total, out_cap);
         }
@@ -609,11 +682,15 @@ static int batch_host_impl(b200timg_ctx *ctx, const b200timg_batch *b, const uin
 
 int b200timg_blocks_batch(b200timg_ctx *ctx, const b200timg_batch *b, const uint8_t *src, char *out,
                           size_t out_cap, uint64_t *offsets) {
-    return batch_host(ctx, b, src, out, out_cap, offsets, false);
+    return batch_host(ctx, b, src, out, out_cap, offsets, Encoder::blocks);
 }
 int b200timg_sixel_batch(b200timg_ctx *ctx, const b200timg_batch *b, const uint8_t *src, char *out,
                          size_t out_cap, uint64_t *offsets) {
-    return batch_host(ctx, b, src, out, out_cap, offsets, true);
+    return batch_host(ctx, b, src, out, out_cap, offsets, Encoder::sixel);
+}
+int b200timg_graphics_batch(b200timg_ctx *ctx, const b200timg_batch *b, const b200timg_graphics *g, const uint8_t *src,
+                            char *out, size_t out_cap, uint64_t *offsets) {
+    return batch_host(ctx, b, src, out, out_cap, offsets, Encoder::graphics, g);
 }
 
 }  // extern "C"

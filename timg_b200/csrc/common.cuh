@@ -89,6 +89,12 @@ struct b200timg_ctx {
     b200timg::DevBuf scale_tmp;    // float4 intermediate + flags of the two-pass scaler (long filters)
     b200timg::DevBuf scale_list;   // work list of tiles the opaque-only scaler hands to the general one
     b200timg::HostBuf pinned;      // staging for sizes / offsets
+    b200timg::DevBuf png_sums;     // per frame: Adler-32 and IDAT CRC-32 of the PNG (png.cu)
+    b200timg::DevBuf gfx_ids;      // kitty image ids of a graphics batch
+    // offsets + ids of a graphics batch go up from here; a slot is reused once its copy has run (ev_gfx)
+    b200timg::HostBuf gfx_stage[4];
+    cudaEvent_t ev_gfx[4] = {nullptr, nullptr, nullptr, nullptr};
+    int gfx_slot = 0;
     b200timg::HostBuf pinned_io;   // staging for pageable payloads
     // host-batch pipeline: upload of chunk k+1 / download of chunk k-1 overlap the kernels of chunk k
     cudaStream_t copy_stream = nullptr, d2h_stream = nullptr;
@@ -241,6 +247,9 @@ int launch_sixel(b200timg_ctx *ctx, const uint8_t *d_fb, int w, int h, int n_fra
                  size_t out_cap, uint64_t *d_offsets, int phases);
 int launch_sixel_front(b200timg_ctx *ctx, const uint8_t *d_fb, int w, int h, int n_total, int f0, int n, bool reserve);
 int launch_sixel_back(b200timg_ctx *ctx, int w, int h, int n_frames, char *d_out, size_t out_cap, uint64_t *d_offsets, int phases);
+// kitty / iTerm2 text of n composed frames at d_out + d_offsets[f] (png.cu); d_ids: kitty image ids
+int launch_graphics(b200timg_ctx *ctx, const uint8_t *d_frames, int w, int h, int n_frames, int rgb24, int protocol,
+                    const uint32_t *d_ids, const uint64_t *d_offsets, char *d_out, size_t out_cap);
 int sixel_debug_fetch(b200timg_ctx *ctx, uint32_t *h_palette, uint32_t *h_counts, uint8_t *h_index, size_t index_bytes);
 
 }  // namespace b200timg
