@@ -18,7 +18,7 @@ LIB_PATH = os.environ.get("B200TIMG_LIBFILE") or os.path.join(_HERE, "libb200tim
 OK, EINVAL, ENOMEM, ECUDA, ENOSPC, ENODEV = 0, -1, -2, -3, -4, -5
 QUARTER, UPPER, COLOR8, FAST_SCALE, BILINEAR_SCALE = 1, 2, 4, 8, 16
 FMT_RGBA, FMT_RGB32, FMT_I420, FMT_NV12, FMT_FULL_RANGE = 0, 1, 2, 3, 0x10
-KITTY, ITERM2 = 1, 2
+KITTY, ITERM2, KITTY_TMUX = 1, 2, 4
 
 u8p = C.POINTER(C.c_uint8)
 u64p = C.POINTER(C.c_uint64)
@@ -38,7 +38,8 @@ class Batch(C.Structure):
 
 
 class Graphics(C.Structure):
-    _fields_ = [("protocol", C.c_int), ("rgb24", C.c_int), ("ids", C.POINTER(C.c_uint32))]
+    _fields_ = [("protocol", C.c_int), ("rgb24", C.c_int), ("ids", C.POINTER(C.c_uint32)),
+                ("cell_x_px", C.c_int), ("cell_y_px", C.c_int), ("indent_cells", C.c_int)]
 
 
 # name -> (restype, argtypes); this table IS the list of exported symbols tests check.
@@ -172,16 +173,19 @@ def resample_plan(iw, ih, ow, oh, axis):
                 coeff=coeff.reshape(n, widest.value))
 
 
-def graphics(protocol, rgb24=False, ids=None):
-    """(b200timg_graphics, the uint32 id array it points to): keep both alive for the call."""
+def graphics(protocol, rgb24=False, ids=None, cell=None, indent=0):
+    """(b200timg_graphics, the uint32 id array it points to): keep both alive for the call.
+    cell=(cell_x_px, cell_y_px) and indent (cells) place the KITTY_TMUX form's placeholder grid."""
     arr = None if ids is None else np.ascontiguousarray(ids, dtype=np.uint32)
-    g = Graphics(protocol, int(rgb24), arr.ctypes.data_as(C.POINTER(C.c_uint32)) if arr is not None else None)
+    cx, cy = cell if cell is not None else (0, 0)
+    g = Graphics(protocol, int(rgb24), arr.ctypes.data_as(C.POINTER(C.c_uint32)) if arr is not None else None,
+                 cx, cy, indent)
     return g, arr
 
 
-def graphics_size(protocol, w, h, rgb24=False, id=0):
-    """Exact bytes of one framed kitty / iTerm2 frame (host only)."""
-    g, _ = graphics(protocol, rgb24)
+def graphics_size(protocol, w, h, rgb24=False, id=0, cell=None, indent=0):
+    """Exact bytes of one framed kitty / iTerm2 frame (host only); 0 for invalid arguments."""
+    g, _ = graphics(protocol, rgb24, cell=cell, indent=indent)
     return lib().b200timg_graphics_size(C.byref(g), w, h, id)
 
 
@@ -349,12 +353,12 @@ class Context:
     def sixel_batch(self, frames, b):
         return self._batch_host(lib().b200timg_sixel_batch, frames, b, sixel=True)
 
-    def graphics_batch(self, frames, b, protocol, rgb24=False, ids=None, with_offsets=False):
-        """Framed kitty / iTerm2 text of every frame (list of bytes); ids: one kitty image id per frame.
-        frames: numpy source frames (RGBA [n,h,w,4], or flat YUV bytes per frame)."""
+    def graphics_batch(self, frames, b, protocol, rgb24=False, ids=None, with_offsets=False, cell=None, indent=0):
+        """Framed kitty / iTerm2 text of every frame (list of bytes); ids: one kitty image id per frame; cell and
+        indent: see graphics().  frames: numpy source frames (RGBA [n,h,w,4], or flat YUV bytes per frame)."""
         frames = np.ascontiguousarray(frames, dtype=np.uint8)
         n = b.n_frames
-        g, keep = graphics(protocol, rgb24, ids)
+        g, keep = graphics(protocol, rgb24, ids, cell, indent)
         sizes = [lib().b200timg_graphics_size(C.byref(g), b.out_w, b.out_h, int(keep[f]) if keep is not None else 0)
                  for f in range(n)]
         cap = max(1, sum(sizes))
@@ -365,11 +369,12 @@ class Context:
         res = [out[int(offs[i]):int(offs[i + 1])].tobytes() for i in range(n)]
         return (res, offs) if with_offsets else res
 
-    def graphics_batch_dev(self, d_src, b, protocol, rgb24=False, ids=None, d_out=None, out_cap=None, d_offsets=None):
+    def graphics_batch_dev(self, d_src, b, protocol, rgb24=False, ids=None, d_out=None, out_cap=None, d_offsets=None,
+                           cell=None, indent=0):
         """Device-resident variant on torch CUDA tensors: returns (d_out, d_offsets) after the (asynchronous) call;
         allocates them when not given (out_cap defaults to the exact size of the batch)."""
         import torch
-        g, keep = graphics(protocol, rgb24, ids)
+        g, keep = graphics(protocol, rgb24, ids, cell, indent)
         n = b.n_frames
         if d_out is None:
             need = sum(lib().b200timg_graphics_size(C.byref(g), b.out_w, b.out_h, int(keep[f]) if keep is not None else 0)

@@ -510,8 +510,12 @@ int b200timg_sixel_batch_dev(b200timg_ctx *ctx, const b200timg_batch *b, const u
 // ---- kitty / iTerm2 batches ------------------------------------------------------------------
 static int validate_graphics(b200timg_ctx *ctx, const b200timg_batch *b, const b200timg_graphics *g) {
     if (!g) return ctx->fail(B200TIMG_EINVAL, "graphics: null protocol description");
-    if (g->protocol != B200TIMG_KITTY && g->protocol != B200TIMG_ITERM2) return ctx->fail(B200TIMG_EINVAL, "graphics: unknown protocol %d", g->protocol);
-    if (g->protocol == B200TIMG_KITTY && !g->ids) return ctx->fail(B200TIMG_EINVAL, "graphics: kitty needs one image id per frame (ids is NULL)");
+    if (g->protocol != B200TIMG_KITTY && g->protocol != B200TIMG_ITERM2 && g->protocol != B200TIMG_KITTY_TMUX)
+        return ctx->fail(B200TIMG_EINVAL, "graphics: unknown protocol %d", g->protocol);
+    if (g->protocol != B200TIMG_ITERM2 && !g->ids) return ctx->fail(B200TIMG_EINVAL, "graphics: kitty needs one image id per frame (ids is NULL)");
+    if (g->protocol == B200TIMG_KITTY_TMUX && (g->cell_x_px <= 0 || g->cell_y_px <= 0 || g->indent_cells < 0))
+        return ctx->fail(B200TIMG_EINVAL, "graphics: tmux placeholders need a positive cell size and indent >= 0 (cell %dx%d, indent %d)",
+                         g->cell_x_px, g->cell_y_px, g->indent_cells);
     if (b->animation != 0) return ctx->fail(B200TIMG_EINVAL, "graphics: kitty / iTerm2 frames have no delta encoding (animation must be 0)");
     if (b200timg_png_size(b->out_w, b->out_h, g->rgb24) > 0x7fffffffu)
         return ctx->fail(B200TIMG_EINVAL, "graphics: the PNG of a %dx%d frame does not fit one IDAT chunk", b->out_w, b->out_h);
@@ -521,7 +525,7 @@ static int validate_graphics(b200timg_ctx *ctx, const b200timg_batch *b, const b
 // offsets[0..n]: the running sum of the frame sizes
 static void graphics_offsets(const b200timg_batch *b, const b200timg_graphics *g, uint64_t *offsets) {
     offsets[0] = 0;
-    const bool kitty = g->protocol == B200TIMG_KITTY;
+    const bool kitty = g->protocol != B200TIMG_ITERM2;
     for (int f = 0; f < b->n_frames; ++f) offsets[f + 1] = offsets[f] + b200timg_graphics_size(g, b->out_w, b->out_h, kitty ? g->ids[f] : 0);
 }
 
@@ -532,7 +536,7 @@ int b200timg_graphics_batch_dev(b200timg_ctx *ctx, const b200timg_batch *b, cons
     if (!d_src || !d_out || !d_offsets) return ctx->fail(B200TIMG_EINVAL, "batch: null pointer");
     B2_TRY(validate_graphics(ctx, b, g));
     const int n = b->n_frames;
-    const bool kitty = g->protocol == B200TIMG_KITTY;
+    const bool kitty = g->protocol != B200TIMG_ITERM2;           // either kitty form: image ids go up too
     // offsets (and kitty's ids) are computed here and go up from a pinned slot; the slot is only rewritten once the
     // copy that last read it has run, which never waits unless four batches are queued behind each other
     const int slot = ctx->gfx_slot;
@@ -557,7 +561,7 @@ int b200timg_graphics_batch_dev(b200timg_ctx *ctx, const b200timg_batch *b, cons
     const ComposeSpec cs = make_compose_spec(b->has_bg, b->bg, b->pattern, b->pattern_w, b->pattern_h);
     B2_TRY(batch_scale(ctx, b, d_src, d_fb, b->out_h, &cs));
     if (ctx->ev_after_scale) B2_CUDA(ctx, cudaEventRecord(ctx->ev_after_scale, ctx->stream));
-    return launch_graphics(ctx, d_fb, b->out_w, b->out_h, n, g->rgb24, g->protocol, ctx->gfx_ids.as<uint32_t>(), d_offsets, d_out, out_cap);
+    return launch_graphics(ctx, d_fb, b->out_w, b->out_h, n, *g, ctx->gfx_ids.as<uint32_t>(), d_offsets, d_out, out_cap);
 }
 
 static int pipe_init(b200timg_ctx *ctx) {
@@ -645,7 +649,16 @@ static int batch_host_impl(b200timg_ctx *ctx, const b200timg_batch *b, const uin
         B2_CUDA(ctx, ctx->pipe_out[i].reserve(blocks_bound));
         ctx->ev_after_scale = ctx->ev_scaled[i];                                   // recorded once pipe_in[i] has been consumed
         b200timg_graphics sub_gfx = {};
-        if (graphics) { sub_gfx = *gfx; if (gfx->ids) sub_gfx.ids = gfx->ids + f0; }
+        if (graphics) {                                        // field by field: the tmux fields exist only where they are read
+            sub_gfx.protocol = gfx->protocol;
+            sub_gfx.rgb24 = gfx->rgb24;
+            sub_gfx.ids = gfx->ids ? gfx->ids + f0 : nullptr;
+            if (gfx->protocol == B200TIMG_KITTY_TMUX) {
+                sub_gfx.cell_x_px = gfx->cell_x_px;
+                sub_gfx.cell_y_px = gfx->cell_y_px;
+                sub_gfx.indent_cells = gfx->indent_cells;
+            }
+        }
         const int rc_k = sixel ? sixel_batch_phases(ctx, &sub, d_in, ctx->pipe_out[i].as<char>(), blocks_bound, ctx->offsets.as<uint64_t>(), 3)
                        : graphics ? b200timg_graphics_batch_dev(ctx, &sub, &sub_gfx, d_in, ctx->pipe_out[i].as<char>(), blocks_bound,
                                                                 ctx->offsets.as<uint64_t>())

@@ -248,7 +248,7 @@ int launch_sixel(b200timg_ctx *ctx, const uint8_t *d_fb, int w, int h, int n_fra
 int launch_sixel_front(b200timg_ctx *ctx, const uint8_t *d_fb, int w, int h, int n_total, int f0, int n, bool reserve);
 int launch_sixel_back(b200timg_ctx *ctx, int w, int h, int n_frames, char *d_out, size_t out_cap, uint64_t *d_offsets, int phases);
 // kitty / iTerm2 text of n composed frames at d_out + d_offsets[f] (png.cu); d_ids: kitty image ids
-int launch_graphics(b200timg_ctx *ctx, const uint8_t *d_frames, int w, int h, int n_frames, int rgb24, int protocol,
+int launch_graphics(b200timg_ctx *ctx, const uint8_t *d_frames, int w, int h, int n_frames, const b200timg_graphics &gr,
                     const uint32_t *d_ids, const uint64_t *d_offsets, char *d_out, size_t out_cap);
 int sixel_debug_fetch(b200timg_ctx *ctx, uint32_t *h_palette, uint32_t *h_counts, uint8_t *h_index, size_t index_bytes);
 

@@ -3,16 +3,18 @@
 
   python tools/bench_graphics.py [--steps K] [--warmup W] [--only NAME]
 
-  C2-kitty    3840x2160 RGBA -> 2700x1519 (C2 geometry), 132 frames, kitty, rgb24 (PNG colour type 2)
-  C2-iterm2   the same through iTerm2
-  C4-kitty    3840x2160 RGBA -> 337x190 (C4 geometry), 128 frames, kitty, rgb24, composed onto black
+  C2-kitty       3840x2160 RGBA -> 2700x1519 (C2 geometry), 132 frames, kitty, rgb24 (PNG colour type 2)
+  C2-kitty-tmux  the same in kitty's tmux form at 9x18-px cells: passthrough framing and a 300 x 85 placeholder grid
+  C2-iterm2      the same through iTerm2
+  C4-kitty       3840x2160 RGBA -> 337x190 (C4 geometry), 128 frames, kitty, rgb24, composed onto black
 
 Per configuration: device-resident Mpx/s of input pixels and encoded GB/s; B_alg = (source bytes + encoded bytes)
 over the chain time, as a share of the H100 SXM's 3350 GB/s (DESIGN.md section 4); the per-kernel ms of one batch
 (b200timg_profile); the host-buffer end-to-end rate (b200timg_graphics_batch: source upload, kernels, download of
 the framed text); and beside it the route that existed before: scale + compose + b200timg_png_batch_dev (unframed
 PNG + base64 on the device), download of both, framing on the host (numpy).  That route starts from frames already
-on the device, so its end-to-end time has no source upload in it.  The GPU's name, power limit and max SM clock are read in the same run.
+on the device, so its end-to-end time has no source upload in it.  The tmux form never had such a route (its
+placeholder grid was not built anywhere), so its png_batch_route is null.  The GPU's name, power limit and max SM clock are read in the same run.
 """
 import argparse
 import ctypes as C
@@ -31,8 +33,10 @@ import timg_b200  # noqa: E402
 from timg_b200 import synth  # noqa: E402
 
 HBM_GBS = 3350.0
+PROTOCOL_NAMES = {timg_b200.KITTY: "kitty", timg_b200.ITERM2: "iterm2", timg_b200.KITTY_TMUX: "kitty-tmux"}
 CONFIGS = {
     "C2-kitty": dict(iw=3840, ih=2160, ow=2700, oh=1519, n=132, proto=timg_b200.KITTY, has_bg=0),
+    "C2-kitty-tmux": dict(iw=3840, ih=2160, ow=2700, oh=1519, n=132, proto=timg_b200.KITTY_TMUX, has_bg=0, cell=(9, 18)),
     "C2-iterm2": dict(iw=3840, ih=2160, ow=2700, oh=1519, n=132, proto=timg_b200.ITERM2, has_bg=0),
     "C4-kitty": dict(iw=3840, ih=2160, ow=337, oh=190, n=128, proto=timg_b200.KITTY, has_bg=1),
 }
@@ -81,7 +85,7 @@ def run(name, cfg, steps, warmup, torch):
                         bg=timg_b200.rgba_u32(0, 0, 0), pattern=0, pattern_w=0, pattern_h=0, flags=0, x_indent_cells=0,
                         animation=0)
     ids = np.arange(1, n + 1, dtype=np.uint32) + np.uint32(1_700_000_000)
-    g, keep = timg_b200.graphics(proto, True, ids)
+    g, keep = timg_b200.graphics(proto, True, ids, cfg.get("cell"))
     d_src = frames_on_device(torch, iw, ih, n)
     total = sum(L.b200timg_graphics_size(C.byref(g), ow, oh, int(i)) for i in ids)
     d_out = torch.empty(total, dtype=torch.uint8, device="cuda")
@@ -116,6 +120,15 @@ def run(name, cfg, steps, warmup, torch):
                                            offs.ctypes.data))
     host_s = (time.perf_counter() - t0) / steps
     same = out.tobytes() == d_out.cpu().numpy().tobytes()
+    result = dict(config=name, frames=n, src=f"{iw}x{ih}", out=f"{ow}x{oh}", protocol=PROTOCOL_NAMES[proto],
+                  rgb24=True, has_bg=bool(cfg["has_bg"]), encoded_bytes=total, steps=steps,
+                  dev_ms=round(ms, 3), dev_mpx_s=round(n * iw * ih / ms / 1e3, 1), dev_encoded_gbs=round(total / ms / 1e6, 2),
+                  b_alg_gbs=round((src_bytes + total) / ms / 1e6, 1), b_alg_share=round((src_bytes + total) / ms / 1e6 / HBM_GBS, 4),
+                  kernels_ms=kernels, host_e2e_ms=round(host_s * 1e3, 2), host_e2e_mpx_s=round(n * iw * ih / host_s / 1e6, 1),
+                  host_equals_dev=same, png_batch_route=None)
+    if proto == timg_b200.KITTY_TMUX:
+        ctx.close()
+        return result
 
     # the earlier route: scale + compose, png_batch_dev (PNG + base64), both downloaded, framed on the host
     png_len = L.b200timg_png_size(ow, oh, 1)
@@ -148,15 +161,10 @@ def run(name, cfg, steps, warmup, torch):
     route_e2e_s = (time.perf_counter() - t0) / steps
     route_same = b"".join(texts) == out.tobytes()
     ctx.close()
-    return dict(config=name, frames=n, src=f"{iw}x{ih}", out=f"{ow}x{oh}", protocol="kitty" if proto == 1 else "iterm2",
-                rgb24=True, has_bg=bool(cfg["has_bg"]), encoded_bytes=total, steps=steps,
-                dev_ms=round(ms, 3), dev_mpx_s=round(n * iw * ih / ms / 1e3, 1), dev_encoded_gbs=round(total / ms / 1e6, 2),
-                b_alg_gbs=round((src_bytes + total) / ms / 1e6, 1), b_alg_share=round((src_bytes + total) / ms / 1e6 / HBM_GBS, 4),
-                kernels_ms=kernels, host_e2e_ms=round(host_s * 1e3, 2), host_e2e_mpx_s=round(n * iw * ih / host_s / 1e6, 1),
-                host_equals_dev=same,
-                png_batch_route=dict(dev_ms=round(route_ms, 3), d2h_bytes=n * (png_len + b64_len),
+    result["png_batch_route"] = dict(dev_ms=round(route_ms, 3), d2h_bytes=n * (png_len + b64_len),
                                      e2e_ms=round(route_e2e_s * 1e3, 2), e2e_mpx_s=round(n * iw * ih / route_e2e_s / 1e6, 1),
-                                     same_bytes=route_same))
+                                     same_bytes=route_same)
+    return result
 
 
 def main():
