@@ -18,6 +18,19 @@ LIB_PATH = os.environ.get("B200TIMG_LIBFILE") or os.path.join(_HERE, "libb200tim
 OK, EINVAL, ENOMEM, ECUDA, ENOSPC, ENODEV = 0, -1, -2, -3, -4, -5
 QUARTER, UPPER, COLOR8, FAST_SCALE, BILINEAR_SCALE = 1, 2, 4, 8, 16
 FMT_RGBA, FMT_RGB32, FMT_I420, FMT_NV12, FMT_FULL_RANGE = 0, 1, 2, 3, 0x10
+FMT_I422, FMT_I444, FMT_I440, FMT_I420_10, FMT_I422_10, FMT_I444_10, FMT_P010 = 4, 5, 6, 7, 8, 9, 10
+YUV_FORMATS = (FMT_I420, FMT_NV12, FMT_I422, FMT_I444, FMT_I440, FMT_I420_10, FMT_I422_10, FMT_I444_10, FMT_P010)
+# low nibble -> (chroma shift x, chroma shift y, bytes per sample): the tightly packed layouts of include/b200timg.h
+_YUV_LAYOUT = {FMT_I420: (1, 1, 1), FMT_NV12: (1, 1, 1), FMT_I422: (1, 0, 1), FMT_I444: (0, 0, 1), FMT_I440: (0, 1, 1),
+               FMT_I420_10: (1, 1, 2), FMT_I422_10: (1, 0, 2), FMT_I444_10: (0, 0, 2), FMT_P010: (1, 1, 2)}
+
+
+def yuv_frame_bytes(fmt, w, h):
+    """Bytes of one tightly packed frame of a YUV format (FULL_RANGE bit ignored), as the library computes them."""
+    sx, sy, bps = _YUV_LAYOUT[fmt & 0xF]
+    return bps * (w * h + 2 * (w >> sx) * (h >> sy))
+
+
 KITTY, ITERM2, KITTY_TMUX = 1, 2, 4
 
 u8p = C.POINTER(C.c_uint8)
@@ -193,6 +206,15 @@ def _np_ptr(a):
     return a.ctypes.data_as(u8p)
 
 
+def _source_frames(frames):
+    """Batch sources as contiguous bytes, frame-major: RGBA [n,h,w,4] uint8, or one flat YUV frame per row in uint8
+    or uint16 samples (the 10-bit formats), reinterpreted bytewise, never converted."""
+    frames = np.ascontiguousarray(frames)
+    if frames.dtype == np.uint16:
+        return frames.reshape(frames.shape[0], -1).view(np.uint8)
+    return np.ascontiguousarray(frames, dtype=np.uint8)
+
+
 class Context:
     """One b200timg_ctx.  Raises B200Error(ENODEV) when no CUDA device is usable."""
 
@@ -230,9 +252,14 @@ class Context:
         return out
 
     def yuv_scale(self, yuv, iw, ih, ow, oh, fmt=FMT_I420):
-        """yuv: flat uint8 array of iw*ih*3/2 bytes (I420 or NV12) -> RGBA [oh, ow, 4]."""
-        yuv = np.ascontiguousarray(yuv, dtype=np.uint8).reshape(-1)
-        assert yuv.size == iw * ih * 3 // 2
+        """yuv: one frame of a YUV format as a flat uint8 or uint16 array (uint16 for the 10-bit formats' samples)
+        whose byte size is the format's layout (I420 / NV12: iw*ih*3/2 bytes) -> RGBA [oh, ow, 4]."""
+        yuv = np.ascontiguousarray(yuv).reshape(-1)
+        if yuv.dtype not in (np.uint8, np.uint16):
+            raise TypeError(f"yuv_scale: uint8 or uint16 samples, not {yuv.dtype}")
+        yuv = yuv.view(np.uint8)
+        if (fmt & 0xF) in _YUV_LAYOUT and yuv.size != yuv_frame_bytes(fmt, iw, ih):
+            raise B200Error(EINVAL, f"yuv_scale: {yuv.size} bytes, format {fmt} at {iw}x{ih} has {yuv_frame_bytes(fmt, iw, ih)}")
         out = np.empty((oh, ow, 4), np.uint8)
         self._chk(lib().b200timg_yuv_scale(self.h, _np_ptr(yuv), iw, ih, fmt, _np_ptr(out), ow, oh))
         return out
@@ -336,7 +363,7 @@ class Context:
 
     # ---- batches, host buffers (numpy [n,h,w,4]) -> list of bytes
     def _batch_host(self, fn, frames, b, sixel=False):
-        frames = np.ascontiguousarray(frames, dtype=np.uint8)
+        frames = _source_frames(frames)
         n = frames.shape[0]
         if sixel:
             cap = n * (4096 + 6 * b.out_w * (b.out_h + 5))      # far above typical (~1 B/px); ENOSPC reports the need
@@ -355,8 +382,9 @@ class Context:
 
     def graphics_batch(self, frames, b, protocol, rgb24=False, ids=None, with_offsets=False, cell=None, indent=0):
         """Framed kitty / iTerm2 text of every frame (list of bytes); ids: one kitty image id per frame; cell and
-        indent: see graphics().  frames: numpy source frames (RGBA [n,h,w,4], or flat YUV bytes per frame)."""
-        frames = np.ascontiguousarray(frames, dtype=np.uint8)
+        indent: see graphics().  frames: numpy source frames (RGBA [n,h,w,4], or one flat YUV frame per row, uint8 or
+        uint16 samples)."""
+        frames = _source_frames(frames)
         n = b.n_frames
         g, keep = graphics(protocol, rgb24, ids, cell, indent)
         sizes = [lib().b200timg_graphics_size(C.byref(g), b.out_w, b.out_h, int(keep[f]) if keep is not None else 0)

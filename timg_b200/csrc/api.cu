@@ -323,10 +323,10 @@ int b200timg_scale_rgba_mode(b200timg_ctx *ctx, const uint8_t *in, int iw, int i
 
 int b200timg_yuv_scale(b200timg_ctx *ctx, const uint8_t *in, int iw, int ih, int fmt, uint8_t *out, int ow, int oh) {
     B2_TRY(check_ctx(ctx));
-    const int f = fmt & 0xf;
-    if (!in || !out || iw <= 0 || ih <= 0 || ow <= 0 || oh <= 0 || (f != B200TIMG_FMT_I420 && f != B200TIMG_FMT_NV12))
+    if (!in || !out || iw <= 0 || ih <= 0 || ow <= 0 || oh <= 0)
         return ctx->fail(B200TIMG_EINVAL, "yuv_scale: bad args");
-    const size_t ib = (size_t)iw * ih + 2 * (size_t)(iw / 2) * (ih / 2), ob = (size_t)ow * oh * 4;
+    B2_TRY(yuv_check_format(ctx, fmt, iw, ih));
+    const size_t ib = (size_t)yuv_frame_bytes(fmt, iw, ih), ob = (size_t)ow * oh * 4;
     B2_CUDA(ctx, ctx->in_stage.reserve(ib));
     ctx->resident_fb = nullptr;
     B2_CUDA(ctx, ctx->fb_scaled.reserve(ob));
@@ -384,8 +384,7 @@ static int validate_batch(b200timg_ctx *ctx, const b200timg_batch *b) {
 }
 
 static size_t src_frame_bytes(const b200timg_batch *b) {
-    const int f = b->src_fmt & 0xf;
-    if (f == B200TIMG_FMT_I420 || f == B200TIMG_FMT_NV12) return (size_t)b->src_w * b->src_h + 2 * (size_t)(b->src_w / 2) * (b->src_h / 2);
+    if (const long long yuv = yuv_frame_bytes(b->src_fmt, b->src_w, b->src_h)) return (size_t)yuv;
     return (size_t)b->src_w * b->src_h * 4;
 }
 
@@ -394,7 +393,7 @@ static size_t src_frame_bytes(const b200timg_batch *b) {
 static int batch_scale(b200timg_ctx *ctx, const b200timg_batch *b, const uint8_t *d_src, uint8_t *d_fb, int frame_rows,
                        const ComposeSpec *cs) {
     const int f = b->src_fmt & 0xf;
-    if (f == B200TIMG_FMT_I420 || f == B200TIMG_FMT_NV12)
+    if (yuv_frame_bytes(b->src_fmt, 2, 2))
         return launch_yuv_scale(ctx, d_src, b->src_w, b->src_h, b->src_fmt, d_fb, b->out_w, b->out_h, frame_rows, b->n_frames);
     if (f != B200TIMG_FMT_RGBA && f != B200TIMG_FMT_RGB32) return ctx->fail(B200TIMG_EINVAL, "batch: unknown source format %d", b->src_fmt);
     if (b->flags & B200TIMG_BILINEAR_SCALE)

@@ -9,14 +9,16 @@
 // distance to the libswscale 9.1 that happens to be bundled with the image's OpenCV wheel (tolerance stated
 // there), plus bit-level agreement with a float64 numpy statement of the same filter to within 1 LSB.
 //
-//   yuv420_rgba_kernel   planar I420 or semi-planar NV12 frame -> RGBA at ow x oh: colour conversion fused
-//                        into the resampler, the RGBA source-size intermediate never exists (SURVEY 8f rank 1).
-//                        1.5 B/px cross PCIe instead of 4.
+//   yuv_rgba_kernel<F>   decoder YUV frame (8-bit 4:2:0 I420 / NV12, 4:2:2, 4:4:4, 4:4:0, 10-bit 4:2:0 / 4:2:2 /
+//                        4:4:4 planar and P010) -> RGBA at ow x oh: colour conversion fused into the resampler, the
+//                        RGBA source-size intermediate never exists (SURVEY 8f rank 1).  1.5-6 B/px cross PCIe
+//                        instead of 4 plus a host conversion pass.  One instantiation per format (YuvFmt).
 //   bilinear_rgba_kernel RGBA -> RGBA triangle filter (the a3 row).
 // One thread per output pixel; taps come from per-axis tables built on the host.  Algorithmic bytes:
 // source bytes read once + 4*ow*oh written.
 #include <algorithm>
 #include <cmath>
+#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
@@ -50,108 +52,150 @@ static void build_tri_axis(int src, int dst, TriAxis *t) {
 struct TriDev { const int32_t *first, *count; const float *coeff; int widest; };
 
 struct YuvParams {
-    int iw, ih, ow, oh, out_frame_rows, nv12, full_range;
+    int iw, ih, ow, oh, out_frame_rows, full_range;
     long long frame_bytes;
     TriDev yh, yv, ch, cv;
 };
 
+// Compile-time description of a decoder format (the low nibble of B200TIMG_FMT_*): chroma subsampling shifts,
+// 8- or 16-bit samples (10 value bits, low or high), planar or interleaved chroma, and whether chroma is filtered at
+// half the output width (libswscale's packed-RGB writers) or at the full width (its full chroma interpolation, which
+// it switches on for sources without chroma subsampling).
+template <int F> struct YuvFmt {
+    static constexpr int sx = (F == B200TIMG_FMT_I444 || F == B200TIMG_FMT_I440 || F == B200TIMG_FMT_I444_10) ? 0 : 1;
+    static constexpr int sy = (F == B200TIMG_FMT_I422 || F == B200TIMG_FMT_I444 || F == B200TIMG_FMT_I422_10 ||
+                               F == B200TIMG_FMT_I444_10) ? 0 : 1;
+    static constexpr bool wide = F >= B200TIMG_FMT_I420_10;        // 16-bit little-endian samples
+    static constexpr bool high10 = F == B200TIMG_FMT_P010;         // value in bits 6..15, else bits 0..9
+    static constexpr bool semi = F == B200TIMG_FMT_NV12 || F == B200TIMG_FMT_P010;
+    static constexpr bool full = sx == 0 && sy == 0;               // chroma at the full output width
+    using S = typename std::conditional<wide, uint16_t, uint8_t>::type;     // one sample
+    using Q = typename std::conditional<wide, uint2, uint32_t>::type;       // four samples (one staging load)
+    __device__ static __forceinline__ float val(S s) { return (float)(high10 ? (s >> 6) : wide ? (s & 0x3ff) : s); }
+    // two 16-bit samples of a word -> their 10 value bits (identity for bytes)
+    __device__ static __forceinline__ uint32_t bits2(uint32_t w) { return high10 ? (w >> 6) & 0x03ff03ffu : wide ? w & 0x03ff03ffu : w; }
+    __device__ static __forceinline__ uint32_t bits(uint32_t w) { return bits2(w); }
+    __device__ static __forceinline__ uint2 bits(uint2 w) { return make_uint2(bits2(w.x), bits2(w.y)); }
+};
+
 __device__ __forceinline__ uint32_t sat8(float v) { return __float2uint_rn(fminf(fmaxf(v, 0.0f), 255.0f)); }
 
-__global__ void __launch_bounds__(256)
-yuv420_rgba_kernel(const uint8_t *__restrict__ in, uint32_t *__restrict__ out, YuvParams P) {
-    const int ox = blockIdx.x * 32 + (threadIdx.x & 31), oy = blockIdx.y * 8 + (threadIdx.x >> 5), f = blockIdx.z;
-    if (ox >= P.ow || oy >= P.oh) return;
-    const uint8_t *Y = in + (long long)f * P.frame_bytes;
-    const int cw = (P.iw + 1) >> 1, chh = (P.ih + 1) >> 1;
-    const uint8_t *U = Y + (long long)P.iw * P.ih, *V = U + (long long)cw * chh;
-    float y = 0.0f, u = 0.0f, v = 0.0f;
-    {
-        const int x0 = P.yh.first[ox], nx = P.yh.count[ox], y0 = P.yv.first[oy], ny = P.yv.count[oy];
-        const float *hx = P.yh.coeff + (long long)ox * P.yh.widest, *hy = P.yv.coeff + (long long)oy * P.yv.widest;
-        for (int j = 0; j < ny; ++j) {
-            const uint8_t *row = Y + (long long)(y0 + j) * P.iw + x0;
-            float a = 0.0f;
-            for (int i = 0; i < nx; ++i) a = fmaf((float)row[i], hx[i], a);
-            y = fmaf(a, hy[j], y);
-        }
-    }
-    {
-        // libswscale's packed-RGB writers (without SWS_FULL_CHR_H_INT, which the reference does not set) carry chroma at
-        // half the OUTPUT width: the two pixels of an output pair share one chroma sample
-        const int cx = ox >> 1;
-        const int x0 = P.ch.first[cx], nx = P.ch.count[cx], y0 = P.cv.first[oy], ny = P.cv.count[oy];
-        const float *hx = P.ch.coeff + (long long)cx * P.ch.widest, *hy = P.cv.coeff + (long long)oy * P.cv.widest;
-        for (int j = 0; j < ny; ++j) {
-            float au = 0.0f, av = 0.0f;
-            if (P.nv12) {
-                const uint8_t *row = U + ((long long)(y0 + j) * cw + x0) * 2;
-                for (int i = 0; i < nx; ++i) { au = fmaf((float)row[2 * i], hx[i], au); av = fmaf((float)row[2 * i + 1], hx[i], av); }
-            } else {
-                const uint8_t *ru = U + (long long)(y0 + j) * cw + x0, *rv = V + (long long)(y0 + j) * cw + x0;
-                for (int i = 0; i < nx; ++i) { au = fmaf((float)ru[i], hx[i], au); av = fmaf((float)rv[i], hx[i], av); }
-            }
-            u = fmaf(au, hy[j], u); v = fmaf(av, hy[j], v);
-        }
-    }
+// filtered Y, Cb, Cr (8-bit domain) -> packed RGBA
+__device__ __forceinline__ uint32_t yuv_to_rgba(float y, float u, float v, int full_range) {
     float r, g, b;
     u -= 128.0f; v -= 128.0f;
-    if (P.full_range) {                       // JPEG / "yuvj": Y, Cb, Cr over 0..255
+    if (full_range) {                         // JPEG / "yuvj": Y, Cb, Cr over 0..255
         r = y + 1.402f * v; g = y - 0.344136f * u - 0.714136f * v; b = y + 1.772f * u;
     } else {                                  // ITU-R BT.601, Y 16..235, Cb/Cr 16..240 (SWS_CS_DEFAULT)
         const float yl = 1.164383f * (y - 16.0f);
         r = yl + 1.596027f * v; g = yl - 0.391762f * u - 0.812968f * v; b = yl + 2.017232f * u;
     }
-    out[((long long)f * P.out_frame_rows + oy) * P.ow + ox] = pack_rgba(sat8(r), sat8(g), sat8(b), 0xffu);
+    return pack_rgba(sat8(r), sat8(g), sat8(b), 0xffu);
+}
+
+template <int F>
+__global__ void __launch_bounds__(256)
+yuv_rgba_kernel(const uint8_t *__restrict__ in, uint32_t *__restrict__ out, YuvParams P) {
+    using T = YuvFmt<F>;
+    using S = typename T::S;
+    const int ox = blockIdx.x * 32 + (threadIdx.x & 31), oy = blockIdx.y * 8 + (threadIdx.x >> 5), f = blockIdx.z;
+    if (ox >= P.ow || oy >= P.oh) return;
+    const S *Y = reinterpret_cast<const S *>(in + (long long)f * P.frame_bytes);
+    const int cw = P.iw >> T::sx, chh = P.ih >> T::sy;
+    const S *U = Y + (long long)P.iw * P.ih, *V = U + (long long)cw * chh;
+    float y = 0.0f, u = 0.0f, v = 0.0f;
+    {
+        const int x0 = P.yh.first[ox], nx = P.yh.count[ox], y0 = P.yv.first[oy], ny = P.yv.count[oy];
+        const float *hx = P.yh.coeff + (long long)ox * P.yh.widest, *hy = P.yv.coeff + (long long)oy * P.yv.widest;
+        for (int j = 0; j < ny; ++j) {
+            const S *row = Y + (long long)(y0 + j) * P.iw + x0;
+            float a = 0.0f;
+            for (int i = 0; i < nx; ++i) a = fmaf(T::val(row[i]), hx[i], a);
+            y = fmaf(a, hy[j], y);
+        }
+    }
+    {
+        // libswscale's packed-RGB writers (without SWS_FULL_CHR_H_INT, which the reference does not set) carry chroma at
+        // half the OUTPUT width: the two pixels of an output pair share one chroma sample.  4:4:4 sources make it
+        // switch to full chroma interpolation: one chroma sample per output pixel.
+        const int cx = T::full ? ox : ox >> 1;
+        const int x0 = P.ch.first[cx], nx = P.ch.count[cx], y0 = P.cv.first[oy], ny = P.cv.count[oy];
+        const float *hx = P.ch.coeff + (long long)cx * P.ch.widest, *hy = P.cv.coeff + (long long)oy * P.cv.widest;
+        for (int j = 0; j < ny; ++j) {
+            float au = 0.0f, av = 0.0f;
+            if (T::semi) {
+                const S *row = U + ((long long)(y0 + j) * cw + x0) * 2;
+                for (int i = 0; i < nx; ++i) { au = fmaf(T::val(row[2 * i]), hx[i], au); av = fmaf(T::val(row[2 * i + 1]), hx[i], av); }
+            } else {
+                const S *ru = U + (long long)(y0 + j) * cw + x0, *rv = V + (long long)(y0 + j) * cw + x0;
+                for (int i = 0; i < nx; ++i) { au = fmaf(T::val(ru[i]), hx[i], au); av = fmaf(T::val(rv[i]), hx[i], av); }
+            }
+            u = fmaf(au, hy[j], u); v = fmaf(av, hy[j], v);
+        }
+    }
+    if (T::wide) { y *= 0.25f; u *= 0.25f; v *= 0.25f; }      // 10-bit -> 8-bit domain (exact: a power of two)
+    out[((long long)f * P.out_frame_rows + oy) * P.ow + ox] = yuv_to_rgba(y, u, v, P.full_range);
 }
 
 
 // ---- tiled variant: the same filter, separable inside a 64 x 32 output tile -------------------------
 // The per-pixel kernel above redoes the horizontal taps of every source row for every output row that uses
-// it.  Here a tile stages its luma / chroma byte windows in shared memory once, runs the vertical taps into
-// float rows (luma at source width, chroma at half the OUTPUT width after its own horizontal pass order is
-// swapped: vertical first for both), then the horizontal taps, converts and stores.  Needs iw % 8 == 0.
+// it.  Here a tile stages its luma / chroma sample windows in shared memory once (8- or 16-bit samples, the
+// 10 value bits already extracted), runs the vertical taps into float rows (luma at source width, chroma at the
+// chroma plane's width), then the horizontal taps, converts and stores.  Needs iw % 8 == 0 and a source
+// pointer aligned to 8 bytes (8-bit formats) or 16 bytes (16-bit formats): every staging load is then one
+// aligned word of four samples (two words for interleaved chroma).
 constexpr int YT_W = 64, YT_H = 32, YT_NT = 256;
 struct YuvTileGeom { int nix, niy, ncx, ncy; };        // window extents (luma cols/rows, chroma cols/rows), maxima over tiles
 
+template <int F>
 __global__ void __launch_bounds__(YT_NT)
-yuv420_rgba_tiled_kernel(const uint8_t *__restrict__ in, uint32_t *__restrict__ out, YuvParams P, YuvTileGeom G) {
+yuv_rgba_tiled_kernel(const uint8_t *__restrict__ in, uint32_t *__restrict__ out, YuvParams P, YuvTileGeom G) {
+    using T = YuvFmt<F>;
+    using S = typename T::S;
+    using Q = typename T::Q;
     extern __shared__ __align__(16) uint8_t s_yuv[];
     const int tid = threadIdx.x, f = blockIdx.z;
     const int ox0 = blockIdx.x * YT_W, oy0 = blockIdx.y * YT_H;
     const int tw = min(YT_W, P.ow - ox0), th = min(YT_H, P.oh - oy0);
-    const int cxa = ox0 >> 1, ncol = (tw + 1) >> 1;               // output chroma columns of this tile: [cxa, cxa + ncol)
-    const int cw = P.iw >> 1, chh = P.ih >> 1;
-    // window origins (tables are monotone), luma x origin aligned down to 4 bytes, chroma x origin to 4 samples
+    const int cxa = T::full ? ox0 : ox0 >> 1;                     // first output chroma column of this tile
+    const int cw = P.iw >> T::sx, chh = P.ih >> T::sy;
+    // window origins (tables are monotone), x origins aligned down to 4 samples
     const int ix0 = P.yh.first[ox0] & ~3, iy0 = P.yv.first[oy0];
     const int cx0 = P.ch.first[cxa] & ~3, cy0 = P.cv.first[oy0];
-    const int nixw = (G.nix + 7) >> 2, ncxw = (G.ncx + 7) >> 2;   // words per staged row (origin alignment slack included)
-    const int ypitch = nixw * 4, cpitch = ncxw * 4;
-    uint8_t *Yw = s_yuv;                                     // [niy][ypitch]
-    uint8_t *Uw = Yw + G.niy * ypitch, *Vw = Uw + G.ncy * cpitch;   // [ncy][cpitch] each
-    float *TY = reinterpret_cast<float *>(Vw + G.ncy * cpitch + ((16 - ((G.niy * ypitch + 2 * G.ncy * cpitch) & 15)) & 15));   // [YT_H][ypitch]
+    const int nixw = (G.nix + 7) >> 2, ncxw = (G.ncx + 7) >> 2;   // 4-sample words per staged row (origin alignment slack included)
+    const int ypitch = nixw * 4, cpitch = ncxw * 4;               // samples
+    S *Yw = reinterpret_cast<S *>(s_yuv);                         // [niy][ypitch]
+    S *Uw = Yw + G.niy * ypitch, *Vw = Uw + G.ncy * cpitch;       // [ncy][cpitch] each
+    const int staged = (G.niy * ypitch + 2 * G.ncy * cpitch) * (int)sizeof(S);
+    float *TY = reinterpret_cast<float *>(s_yuv + staged + ((16 - (staged & 15)) & 15));   // [YT_H][ypitch]
     float *TU = TY + YT_H * ypitch, *TV = TU + YT_H * cpitch;    // [YT_H][cpitch]
-    const uint8_t *Y = in + (long long)f * P.frame_bytes;
-    const uint8_t *C = Y + (long long)P.iw * P.ih;
+    const S *Y = reinterpret_cast<const S *>(in + (long long)f * P.frame_bytes);
+    const S *C = Y + (long long)P.iw * P.ih;
     for (int u = tid; u < G.niy * nixw; u += YT_NT) {
         const int ly = u / nixw, g = u - ly * nixw, y = iy0 + ly, x = ix0 + 4 * g;
-        uint32_t v = 0;
-        if (y < P.ih && x < P.iw) v = __ldg(reinterpret_cast<const uint32_t *>(Y + (long long)y * P.iw + x));
-        reinterpret_cast<uint32_t *>(Yw + ly * ypitch)[g] = v;
+        Q v{};
+        if (y < P.ih && x < P.iw) v = T::bits(__ldg(reinterpret_cast<const Q *>(Y + (long long)y * P.iw + x)));
+        reinterpret_cast<Q *>(Yw + ly * ypitch)[g] = v;
     }
     for (int u = tid; u < G.ncy * ncxw; u += YT_NT) {
         const int ly = u / ncxw, g = u - ly * ncxw, y = cy0 + ly, x = cx0 + 4 * g;
-        uint32_t pu = 0, pv = 0;
+        Q pu{}, pv{};
         if (y < chh && x < cw) {
-            if (P.nv12) {
+            if constexpr (T::semi && !T::wide) {
                 const uint2 q = __ldg(reinterpret_cast<const uint2 *>(C + ((long long)y * cw + x) * 2));      // U0 V0 U1 V1 | U2 V2 U3 V3
                 pu = __byte_perm(q.x, q.y, 0x6420); pv = __byte_perm(q.x, q.y, 0x7531);
+            } else if constexpr (T::semi) {
+                const uint4 q = __ldg(reinterpret_cast<const uint4 *>(C + ((long long)y * cw + x) * 2));      // U0 V0 | U1 V1 | U2 V2 | U3 V3
+                pu = T::bits(make_uint2(__byte_perm(q.x, q.y, 0x5410), __byte_perm(q.z, q.w, 0x5410)));
+                pv = T::bits(make_uint2(__byte_perm(q.x, q.y, 0x7632), __byte_perm(q.z, q.w, 0x7632)));
             } else {
-                pu = __ldg(reinterpret_cast<const uint32_t *>(C + (long long)y * cw + x));
-                pv = __ldg(reinterpret_cast<const uint32_t *>(C + (long long)cw * chh + (long long)y * cw + x));
+                pu = T::bits(__ldg(reinterpret_cast<const Q *>(C + (long long)y * cw + x)));
+                pv = T::bits(__ldg(reinterpret_cast<const Q *>(C + (long long)cw * chh + (long long)y * cw + x)));
             }
         }
-        reinterpret_cast<uint32_t *>(Uw + ly * cpitch)[g] = pu;
-        reinterpret_cast<uint32_t *>(Vw + ly * cpitch)[g] = pv;
+        reinterpret_cast<Q *>(Uw + ly * cpitch)[g] = pu;
+        reinterpret_cast<Q *>(Vw + ly * cpitch)[g] = pv;
     }
     __syncthreads();
     // vertical taps: luma rows -> TY, chroma rows -> TU / TV
@@ -183,17 +227,13 @@ yuv420_rgba_tiled_kernel(const uint8_t *__restrict__ in, uint32_t *__restrict__ 
             for (int i = 0; i < nx; ++i) y = fmaf(row[i], hx[i], y);
         }
         {
-            const int cx = ox >> 1, x0 = P.ch.first[cx] - cx0, nx = P.ch.count[cx];
+            const int cx = T::full ? ox : ox >> 1, x0 = P.ch.first[cx] - cx0, nx = P.ch.count[cx];
             const float *hx = P.ch.coeff + (long long)cx * P.ch.widest, *ru = TU + ty * cpitch + x0, *rv = TV + ty * cpitch + x0;
             for (int i = 0; i < nx; ++i) { uu = fmaf(ru[i], hx[i], uu); vv = fmaf(rv[i], hx[i], vv); }
         }
-        float r, g, b;
-        uu -= 128.0f; vv -= 128.0f;
-        if (P.full_range) { r = y + 1.402f * vv; g = y - 0.344136f * uu - 0.714136f * vv; b = y + 1.772f * uu; }
-        else { const float yl = 1.164383f * (y - 16.0f); r = yl + 1.596027f * vv; g = yl - 0.391762f * uu - 0.812968f * vv; b = yl + 2.017232f * uu; }
-        out[((long long)f * P.out_frame_rows + oy) * P.ow + ox] = pack_rgba(sat8(r), sat8(g), sat8(b), 0xffu);
+        if (T::wide) { y *= 0.25f; uu *= 0.25f; vv *= 0.25f; }
+        out[((long long)f * P.out_frame_rows + oy) * P.ow + ox] = yuv_to_rgba(y, uu, vv, P.full_range);
     }
-    (void)ncol;
 }
 
 struct BilinearParams { int iw, ih, ow, oh, out_frame_rows, bgra; TriDev h, v; ComposeSpec cs; };
@@ -267,27 +307,66 @@ static int upload_tri(b200timg_ctx *ctx, TriUpload &up) {
     return B200TIMG_OK;
 }
 
-// fmt: B200TIMG_FMT_I420 / _NV12, optionally | B200TIMG_FMT_FULL_RANGE
-int launch_yuv_scale(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int fmt, uint8_t *d_out, int ow, int oh,
-                     int out_frame_rows, int n_frames) {
-    if (out_frame_rows < oh) return ctx->fail(B200TIMG_EINVAL, "yuv: frame rows < out height");
-    if ((iw | ih) & 1) return ctx->fail(B200TIMG_EINVAL, "yuv: 4:2:0 frames need even width and height");
-    if (n_frames > 65535) return ctx->fail(B200TIMG_EINVAL, "yuv: too many frames for one launch");
-    const int cw = iw / 2, ch = ih / 2;
+// Bytes of one tightly packed frame of a YUV format (any FULL_RANGE bit ignored); 0 for a code that is not one.
+long long yuv_frame_bytes(int fmt, int iw, int ih) {
+    const int f = fmt & 0xf;
+    if (f < B200TIMG_FMT_I420 || f > B200TIMG_FMT_P010) return 0;
+    const bool wide = f >= B200TIMG_FMT_I420_10;
+    const int sx = (f == B200TIMG_FMT_I444 || f == B200TIMG_FMT_I440 || f == B200TIMG_FMT_I444_10) ? 0 : 1;
+    const int sy = (f == B200TIMG_FMT_I422 || f == B200TIMG_FMT_I444 || f == B200TIMG_FMT_I422_10 || f == B200TIMG_FMT_I444_10) ? 0 : 1;
+    return (wide ? 2 : 1) * ((long long)iw * ih + 2ll * (iw >> sx) * (ih >> sy));
+}
+
+static const char *yuv_fmt_name(int f) {
+    static const char *const names[] = {"I420", "NV12", "I422", "I444", "I440", "I420_10", "I422_10", "I444_10", "P010"};
+    return f >= B200TIMG_FMT_I420 && f <= B200TIMG_FMT_P010 ? names[f - B200TIMG_FMT_I420] : "?";
+}
+
+// EINVAL unless fmt is a YUV code and iw x ih is a multiple of its chroma subsampling
+int yuv_check_format(b200timg_ctx *ctx, int fmt, int iw, int ih) {
+    const int f = fmt & 0xf;
+    if (!yuv_frame_bytes(fmt, 2, 2)) return ctx->fail(B200TIMG_EINVAL, "yuv: unknown source format %d", fmt);
+    const bool hsub = f != B200TIMG_FMT_I444 && f != B200TIMG_FMT_I440 && f != B200TIMG_FMT_I444_10;
+    const bool vsub = f != B200TIMG_FMT_I422 && f != B200TIMG_FMT_I444 && f != B200TIMG_FMT_I422_10 && f != B200TIMG_FMT_I444_10;
+    if ((hsub && (iw & 1)) || (vsub && (ih & 1)))
+        return ctx->fail(B200TIMG_EINVAL, "yuv: %s frames need an even %s (got %dx%d)", yuv_fmt_name(f),
+                         hsub && vsub ? "width and height" : hsub ? "width" : "height", iw, ih);
+    return B200TIMG_OK;
+}
+
+template <int F> struct YuvKernelName;
+#define B2_YUV_NAMES(F, sfx) template <> struct YuvKernelName<F> { \
+    static constexpr const char *tiled = "yuv_rgba_tiled_kernel_" sfx, *simple = "yuv_rgba_kernel_" sfx; };
+B2_YUV_NAMES(B200TIMG_FMT_I420, "i420") B2_YUV_NAMES(B200TIMG_FMT_NV12, "nv12") B2_YUV_NAMES(B200TIMG_FMT_I422, "i422")
+B2_YUV_NAMES(B200TIMG_FMT_I444, "i444") B2_YUV_NAMES(B200TIMG_FMT_I440, "i440") B2_YUV_NAMES(B200TIMG_FMT_I420_10, "i420_10")
+B2_YUV_NAMES(B200TIMG_FMT_I422_10, "i422_10") B2_YUV_NAMES(B200TIMG_FMT_I444_10, "i444_10") B2_YUV_NAMES(B200TIMG_FMT_P010, "p010")
+#undef B2_YUV_NAMES
+
+template <int F>
+static int launch_yuv_fmt(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int fmt, uint8_t *d_out, int ow, int oh,
+                          int out_frame_rows, int n_frames) {
+    using T = YuvFmt<F>;
+    const int cw = iw >> T::sx, ch = ih >> T::sy, cow = T::full ? ow : (ow + 1) / 2;
+    // libswscale's unscaled yuv2rgb converters exist for 8-bit 4:2:0 only: they replicate chroma rows (2x2 blocks
+    // share a sample); every other format goes through the scaler's triangle filter even at scale 1
+    const bool replicate = (F == B200TIMG_FMT_I420 || F == B200TIMG_FMT_NV12) && ow == iw && oh == ih;
     YuvParams P;
     P.iw = iw; P.ih = ih; P.ow = ow; P.oh = oh; P.out_frame_rows = out_frame_rows;
-    P.nv12 = (fmt & 0xf) == B200TIMG_FMT_NV12; P.full_range = (fmt & B200TIMG_FMT_FULL_RANGE) != 0;
-    P.frame_bytes = (long long)iw * ih + 2ll * cw * ch;
+    P.full_range = (fmt & B200TIMG_FMT_FULL_RANGE) != 0;
+    P.frame_bytes = yuv_frame_bytes(F, iw, ih);
+    // the tables (and the tile extents beside them) depend on the chroma layout, not only on the geometry: it is part
+    // of the cache key.  I420 / NV12 and the other layouts that share tables share an entry.
+    const int kind = 1 | T::sx << 4 | T::sy << 5 | (int)T::full << 6 | (int)(F == B200TIMG_FMT_I420 || F == B200TIMG_FMT_NV12) << 7;
     TriDev td[4];
-    if (!tri_cached(ctx, 1, iw, ih, ow, oh, td, sizeof td)) {
+    if (!tri_cached(ctx, kind, iw, ih, ow, oh, td, sizeof td)) {
         TriAxis yh, yv, chx, cvy;
-        build_tri_axis(iw, ow, &yh); build_tri_axis(ih, oh, &yv); build_tri_axis(cw, (ow + 1) / 2, &chx); build_tri_axis(ch, oh, &cvy);
-        if (ow == iw && oh == ih) {              // no scaling: libswscale's unscaled yuv2rgb path replicates chroma rows (2x2 blocks share a sample)
+        build_tri_axis(iw, ow, &yh); build_tri_axis(ih, oh, &yv); build_tri_axis(cw, cow, &chx); build_tri_axis(ch, oh, &cvy);
+        if (replicate) {
             cvy.widest = 1; cvy.coeff.assign((size_t)oh, 1.0f);
             for (int y = 0; y < oh; ++y) { cvy.first[y] = y >> 1; cvy.count[y] = 1; }
         }
         TriUpload up;
-        up.add(yh, ow, &td[0]); up.add(yv, oh, &td[1]); up.add(chx, (ow + 1) / 2, &td[2]); up.add(cvy, oh, &td[3]);
+        up.add(yh, ow, &td[0]); up.add(yv, oh, &td[1]); up.add(chx, cow, &td[2]); up.add(cvy, oh, &td[3]);
         {   // tile window extents for the tiled kernel
             auto extent = [](const TriAxis &t, int n, int tile, int align) {
                 int best = 1;
@@ -299,37 +378,55 @@ int launch_yuv_scale(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int
                 return best;
             };
             ctx->yuv_geom[0] = extent(yh, ow, YT_W, 4); ctx->yuv_geom[1] = extent(yv, oh, YT_H, 1);
-            ctx->yuv_geom[2] = extent(chx, (ow + 1) / 2, YT_W / 2, 4); ctx->yuv_geom[3] = extent(cvy, oh, YT_H, 1);
+            ctx->yuv_geom[2] = extent(chx, cow, T::full ? YT_W : YT_W / 2, 4); ctx->yuv_geom[3] = extent(cvy, oh, YT_H, 1);
             ctx->yuv_geom_valid = true;
         }
         ctx->tri_key[0] = 0;
         B2_TRY(upload_tri(ctx, up));
         const char *base = ctx->tri_tables.as<char>();
         for (auto &t : td) rebase(&t, base);
-        tri_remember(ctx, 1, iw, ih, ow, oh, td, sizeof td);
+        tri_remember(ctx, kind, iw, ih, ow, oh, td, sizeof td);
     }
     P.yh = td[0]; P.yv = td[1]; P.ch = td[2]; P.cv = td[3];
-    if ((iw & 7) == 0 && (reinterpret_cast<uintptr_t>(d_in) & 7) == 0 && !getenv("B200TIMG_YUV_SIMPLE")) {
+    const uintptr_t align = T::wide ? 15 : 7;
+    if ((iw & 7) == 0 && (reinterpret_cast<uintptr_t>(d_in) & align) == 0 && !getenv("B200TIMG_YUV_SIMPLE") && ctx->yuv_geom_valid) {
         // window extents of a 64 x 32 tile (maxima over tiles), from the host copies of the tables
-        const YuvTileGeom G = ctx->yuv_geom_valid ? YuvTileGeom{ctx->yuv_geom[0], ctx->yuv_geom[1], ctx->yuv_geom[2], ctx->yuv_geom[3]} : YuvTileGeom{0, 0, 0, 0};
-        if (ctx->yuv_geom_valid) {
-            const int nixw = (G.nix + 7) >> 2, ncxw = (G.ncx + 7) >> 2;
-            const size_t bytes = (size_t)G.niy * nixw * 4 + 2 * (size_t)G.ncy * ncxw * 4 + 16 +
-                                 sizeof(float) * ((size_t)YT_H * nixw * 4 + 2 * (size_t)YT_H * ncxw * 4);
-            if (bytes <= 200 * 1024) {
-                B2_CUDA(ctx, cudaFuncSetAttribute(yuv420_rgba_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-                B2_KERNEL(ctx, "yuv420_rgba_tiled_kernel");
-                yuv420_rgba_tiled_kernel<<<dim3((ow + YT_W - 1) / YT_W, (oh + YT_H - 1) / YT_H, n_frames), YT_NT, bytes, ctx->stream>>>(
-                    d_in, reinterpret_cast<uint32_t *>(d_out), P, G);
-                B2_LAUNCH_CHECK(ctx);
-                return B200TIMG_OK;
-            }
+        const YuvTileGeom G{ctx->yuv_geom[0], ctx->yuv_geom[1], ctx->yuv_geom[2], ctx->yuv_geom[3]};
+        const int nixw = (G.nix + 7) >> 2, ncxw = (G.ncx + 7) >> 2;
+        const size_t bytes = ((size_t)G.niy * nixw * 4 + 2 * (size_t)G.ncy * ncxw * 4) * sizeof(typename T::S) + 16 +
+                             sizeof(float) * ((size_t)YT_H * nixw * 4 + 2 * (size_t)YT_H * ncxw * 4);
+        if (bytes <= 200 * 1024) {
+            B2_CUDA(ctx, cudaFuncSetAttribute(yuv_rgba_tiled_kernel<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+            B2_KERNEL(ctx, YuvKernelName<F>::tiled);
+            yuv_rgba_tiled_kernel<F><<<dim3((ow + YT_W - 1) / YT_W, (oh + YT_H - 1) / YT_H, n_frames), YT_NT, bytes, ctx->stream>>>(
+                d_in, reinterpret_cast<uint32_t *>(d_out), P, G);
+            B2_LAUNCH_CHECK(ctx);
+            return B200TIMG_OK;
         }
     }
-    B2_KERNEL(ctx, "yuv420_rgba_kernel");
-    yuv420_rgba_kernel<<<dim3((ow + 31) / 32, (oh + 7) / 8, n_frames), 256, 0, ctx->stream>>>(d_in, reinterpret_cast<uint32_t *>(d_out), P);
+    B2_KERNEL(ctx, YuvKernelName<F>::simple);
+    yuv_rgba_kernel<F><<<dim3((ow + 31) / 32, (oh + 7) / 8, n_frames), 256, 0, ctx->stream>>>(d_in, reinterpret_cast<uint32_t *>(d_out), P);
     B2_LAUNCH_CHECK(ctx);
     return B200TIMG_OK;
+}
+
+// fmt: any B200TIMG_FMT_* YUV code, optionally | B200TIMG_FMT_FULL_RANGE
+int launch_yuv_scale(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int fmt, uint8_t *d_out, int ow, int oh,
+                     int out_frame_rows, int n_frames) {
+    if (out_frame_rows < oh) return ctx->fail(B200TIMG_EINVAL, "yuv: frame rows < out height");
+    B2_TRY(yuv_check_format(ctx, fmt, iw, ih));
+    if (n_frames > 65535) return ctx->fail(B200TIMG_EINVAL, "yuv: too many frames for one launch");
+    switch (fmt & 0xf) {
+    case B200TIMG_FMT_I420: return launch_yuv_fmt<B200TIMG_FMT_I420>(ctx, d_in, iw, ih, fmt, d_out, ow, oh, out_frame_rows, n_frames);
+    case B200TIMG_FMT_NV12: return launch_yuv_fmt<B200TIMG_FMT_NV12>(ctx, d_in, iw, ih, fmt, d_out, ow, oh, out_frame_rows, n_frames);
+    case B200TIMG_FMT_I422: return launch_yuv_fmt<B200TIMG_FMT_I422>(ctx, d_in, iw, ih, fmt, d_out, ow, oh, out_frame_rows, n_frames);
+    case B200TIMG_FMT_I444: return launch_yuv_fmt<B200TIMG_FMT_I444>(ctx, d_in, iw, ih, fmt, d_out, ow, oh, out_frame_rows, n_frames);
+    case B200TIMG_FMT_I440: return launch_yuv_fmt<B200TIMG_FMT_I440>(ctx, d_in, iw, ih, fmt, d_out, ow, oh, out_frame_rows, n_frames);
+    case B200TIMG_FMT_I420_10: return launch_yuv_fmt<B200TIMG_FMT_I420_10>(ctx, d_in, iw, ih, fmt, d_out, ow, oh, out_frame_rows, n_frames);
+    case B200TIMG_FMT_I422_10: return launch_yuv_fmt<B200TIMG_FMT_I422_10>(ctx, d_in, iw, ih, fmt, d_out, ow, oh, out_frame_rows, n_frames);
+    case B200TIMG_FMT_I444_10: return launch_yuv_fmt<B200TIMG_FMT_I444_10>(ctx, d_in, iw, ih, fmt, d_out, ow, oh, out_frame_rows, n_frames);
+    default: return launch_yuv_fmt<B200TIMG_FMT_P010>(ctx, d_in, iw, ih, fmt, d_out, ow, oh, out_frame_rows, n_frames);
+    }
 }
 
 int launch_scale_bilinear(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int fmt, uint8_t *d_out, int ow, int oh,

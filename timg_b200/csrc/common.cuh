@@ -82,9 +82,9 @@ struct b200timg_ctx {
     b200timg::DevBuf sixel_work;   // palettes, LUTs, index planes, band tables
     b200timg::DevBuf misc;         // small flags / sizes
     b200timg::DevBuf tri_tables;   // bilinear / YUV scaler tap tables ...
-    int tri_key[5] = {0, 0, 0, 0, 0};          // ... for this (kind, iw, ih, ow, oh), device pointers cached in tri_params
-    std::vector<char> tri_params;
-    int yuv_geom[4] = {0, 0, 0, 0};            // window extents of the tiled YUV kernel for the cached geometry
+    int tri_key[5] = {0, 0, 0, 0, 0};          // ... for this (kind, iw, ih, ow, oh), device pointers cached in tri_params;
+    std::vector<char> tri_params;              // kind names the scaler and, for YUV, the chroma layout
+    int yuv_geom[4] = {0, 0, 0, 0};            // window extents of the tiled YUV kernel for the cached key
     bool yuv_geom_valid = false;
     b200timg::DevBuf scale_tmp;    // float4 intermediate + flags of the two-pass scaler (long filters)
     b200timg::DevBuf scale_list;   // work list of tiles the opaque-only scaler hands to the general one
@@ -238,9 +238,12 @@ int launch_blocks(b200timg_ctx *ctx, const uint8_t *d_fb, const uint8_t *d_prev,
 // fast != 0: the <= 1 LSB arithmetic (FMA, no 1/255 round trip) where a kernel offers it; 0: bit-exact.
 int launch_scale(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int fmt, uint8_t *d_out,
                  int ow, int oh, int out_frame_rows, int n_frames, const ComposeSpec *cs = nullptr, int fast = 0);
-// libswscale-style bilinear (triangle) scalers, bilinear.cu: RGBA -> RGBA and YUV 4:2:0 -> RGBA
+// libswscale-style bilinear (triangle) scalers, bilinear.cu: RGBA -> RGBA and decoder YUV -> RGBA
 int launch_scale_bilinear(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int fmt, uint8_t *d_out, int ow, int oh,
                           int out_frame_rows, int n_frames, const ComposeSpec *cs);
+// bytes of one tightly packed frame of a YUV B200TIMG_FMT_* code (0 if fmt is not one), and its argument check
+long long yuv_frame_bytes(int fmt, int iw, int ih);
+int yuv_check_format(b200timg_ctx *ctx, int fmt, int iw, int ih);
 int launch_yuv_scale(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int fmt, uint8_t *d_out, int ow, int oh,
                      int out_frame_rows, int n_frames);
 int launch_sixel(b200timg_ctx *ctx, const uint8_t *d_fb, int w, int h, int n_frames, char *d_out,
