@@ -766,6 +766,34 @@ __device__ __forceinline__ void slot_append(uint32_t *slot, uint32_t &pos, uint3
     pos = np;
 }
 
+// Phase clocks of the emit kernels (tools/bench_sixel_emit.py --clocks): built only with -DB200TIMG_EMIT_CLOCKS.  Thread 0
+// stamps clock64() after a CTA barrier at every phase boundary (the instrumented build adds barriers where a phase has
+// none) and adds the CTA's phase durations to g_emit_clocks[kernel][phase]; b200timg_emit_clocks() reads and clears them.
+#ifdef B200TIMG_EMIT_CLOCKS
+constexpr int EMIT_CLK_PHASES = 8;
+__device__ unsigned long long g_emit_clocks[2][EMIT_CLK_PHASES];     // [0: emit1b, 1: emit5][phase], SM cycles summed over CTAs
+#define EMIT_CLK_BEGIN long long clk_[EMIT_CLK_PHASES + 1]; int clk_n_ = 0; if (threadIdx.x == 0) clk_[clk_n_] = clock64(); ++clk_n_
+#define EMIT_CLK() do { __syncthreads(); if (threadIdx.x == 0) clk_[clk_n_] = clock64(); ++clk_n_; } while (0)
+#define EMIT_CLK_END(kern) do { if (threadIdx.x == 0) for (int k_ = 0; k_ + 1 < clk_n_; ++k_) \
+        atomicAdd(&g_emit_clocks[kern][k_], (unsigned long long)(clk_[k_ + 1] - clk_[k_])); } while (0)
+#else
+#define EMIT_CLK_BEGIN do {} while (0)
+#define EMIT_CLK() do {} while (0)
+#define EMIT_CLK_END(kern) do {} while (0)
+#endif
+
+// emit5 (V5) is v1b with two changes, both chosen from v1b's phase clocks (DESIGN.md §5):
+//   * the band's six index rows (one contiguous block of 6*w bytes) come in with coalesced word loads, all in flight at
+//     once and issued before the table zeroing, into the entry array (dead until the scatter); the count pass reads its
+//     columns from there.  v1b's count pass waited for one global round trip per 32-column step.  (w <= 3072 only: wider
+//     bands re-read their columns in the scatter pass, so they keep v1b's loads.)
+//   * the copy-out: when no slot overflowed, every thread moves its slot's bytes to their place in one contiguous byte
+//     image of the band in shared memory (the entry array again), and the CTA writes that image to the 256-byte aligned
+//     scratch slot with 16-byte stores.  v1b's threads each stored their ~32 bytes as 4-byte words, a warp store touching
+//     32 sectors.
+constexpr int ROW_WORDS = (6 * 32 * STASH_STEPS * EW + 3) / 4 / ET + 1;   // words of the staged rows per thread (+1: misalignment)
+
+template <bool V5>
 __global__ void __launch_bounds__(ET, 2)
 sixel_emit1b_kernel(EmitGeom G, SixelWork W) {
     extern __shared__ uint32_t s_sorted[];                   // [6*w]
@@ -774,14 +802,32 @@ sixel_emit1b_kernel(EmitGeom G, SixelWork W) {
     const int band = blockIdx.x, f = blockIdx.y, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const int w = G.w;
     const uint8_t *idx = W.index + ((long long)f * G.h + (long long)band * 6) * w;
-
-    for (int i = tid; i < 2 * EW * 256; i += ET) s_tab[i] = 0;
+    EMIT_CLK_BEGIN;
+    const bool stash = G.cols_per_warp <= 32 * STASH_STEPS;
+    const uint8_t *cols = idx;                               // where the count pass reads the band's rows
+    if (V5 && stash) {
+        // aligned words covering [idx, idx + 6w).  The <= 3 bytes outside the band stay inside the index region: sixel_plan
+        // starts it on a 256-byte boundary and pads its end to one (o_idx, align_up(npix * n_frames, 256)), so rounding
+        // the first band's start down or the last band's end up to a word never leaves it.
+        const uint32_t a = (uint32_t)(reinterpret_cast<uintptr_t>(idx) & 3u);
+        const uint32_t *gw = reinterpret_cast<const uint32_t *>(idx - a);
+        const int nw = (int)((a + 6u * (uint32_t)w + 3u) >> 2);
+        uint32_t rw[ROW_WORDS];
+#pragma unroll
+        for (int k = 0; k < ROW_WORDS; ++k) { const int j = tid + k * ET; rw[k] = j < nw ? gw[j] : 0u; }
+        for (int i = tid; i < 2 * EW * 256; i += ET) s_tab[i] = 0;
+#pragma unroll
+        for (int k = 0; k < ROW_WORDS; ++k) { const int j = tid + k * ET; if (j < nw) s_sorted[j] = rw[k]; }
+        cols = reinterpret_cast<const uint8_t *>(s_sorted) + a;
+    } else {
+        for (int i = tid; i < 2 * EW * 256; i += ET) s_tab[i] = 0;
+    }
     __syncthreads();
+    if (!V5) EMIT_CLK();                                     // zero
     // (1) the sort: as in v1, but the column entries (<= 6 distinct colours of a column with their row bits) are computed
     // once: the count pass parks them in registers (3 words per 32-column step, steps unrolled) for the scatter pass
     const int x_lo = wid * G.cols_per_warp, x_hi = min(w, x_lo + G.cols_per_warp);
     uint32_t *cnt = s_tab + wid * 256, *M = s_tab + EW * 256 + wid * 256;
-    const bool stash = G.cols_per_warp <= 32 * STASH_STEPS;
     uint32_t k0[STASH_STEPS], k1[STASH_STEPS], k2[STASH_STEPS];     // colours 0-3 | colours 4-5, valid, bits 5 | bits 0-4
     if (stash) {
 #pragma unroll
@@ -790,7 +836,7 @@ sixel_emit1b_kernel(EmitGeom G, SixelWork W) {
             k0[t] = k1[t] = k2[t] = 0;
             if (x < x_hi) {
                 uint32_t col[6], bits[6];
-                const uint32_t valid = column_entries(idx, w, x, col, bits);
+                const uint32_t valid = column_entries(cols, w, x, col, bits);
 #pragma unroll
                 for (int s = 0; s < 6; ++s) if (valid & (1u << s)) atomicAdd(&cnt[col[s]], 1u);
                 k0[t] = col[0] | (col[1] << 8) | (col[2] << 16) | (col[3] << 24);
@@ -807,6 +853,7 @@ sixel_emit1b_kernel(EmitGeom G, SixelWork W) {
         }
     }
     __syncthreads();
+    EMIT_CLK();                                              // count
     uint32_t tot_c = 0;
     if (tid < 256) for (int k = 0; k < EW; ++k) tot_c += s_tab[k * 256 + tid];
     uint32_t n_ent; const uint32_t cb = block_excl_scan<ET>(tid < 256 ? tot_c : 0, s_w, n_ent);
@@ -815,6 +862,7 @@ sixel_emit1b_kernel(EmitGeom G, SixelWork W) {
         for (int k = 0; k < EW; ++k) { const uint32_t v = s_tab[k * 256 + tid]; s_tab[k * 256 + tid] = run; run += v; }
     }
     __syncthreads();
+    EMIT_CLK();                                              // offsets
     const uint32_t lt = (1u << lane) - 1;
     auto scatter_step = [&](int x, uint32_t valid, const uint32_t *col, const uint32_t *bits) {
 #pragma unroll
@@ -851,6 +899,7 @@ sixel_emit1b_kernel(EmitGeom G, SixelWork W) {
         }
     }
     __syncthreads();                                         // the tables are dead: s_tab is the slot array from here on
+    EMIT_CLK();                                              // scatter
     // (2) one walk: bytes into the slot, size = the slot's fill
     const int n = (int)n_ent;
     const uint32_t minc = s_sorted[0] >> 18;
@@ -880,25 +929,43 @@ sixel_emit1b_kernel(EmitGeom G, SixelWork W) {
         }
     });
     const uint32_t local = pos;
+    EMIT_CLK();                                              // walk
     uint32_t band_total; const uint32_t at = block_excl_scan<ET>(local, s_w, band_total);
     if (tid == 0) W.band_bytes[(long long)f * W.nbands + band] = band_total;
-    // (3) the slot's bytes into this band's scratch place (16-byte aligned base): head bytes up to a word boundary, whole
-    // words realigned with a funnel shift, tail bytes
-    char *o = W.scratch + ((size_t)f * W.nbands + band) * W.band_cap + at;
-    if (!ovf) {
+    EMIT_CLK();                                              // scan
+    // (3) the slot's bytes to `at` of this band's 16-byte aligned scratch place (v1b), or of its image in shared memory
+    // (emit5): head bytes up to a word boundary, whole words realigned with a funnel shift, tail bytes
+    char *const band_out = W.scratch + ((size_t)f * W.nbands + band) * W.band_cap;
+    char *o = band_out + at;
+    auto slot_out = [&](char *d) {
         const uint32_t head = min(local, (4u - (at & 3u)) & 3u);
         const uint32_t w0 = slot[0];
-        for (uint32_t k = 0; k < head; ++k) o[k] = (char)(w0 >> (8u * k));
+        for (uint32_t k = 0; k < head; ++k) d[k] = (char)(w0 >> (8u * k));
         const uint32_t nw = (local - head) >> 2;
-        uint32_t *dw = reinterpret_cast<uint32_t *>(o + head);
+        uint32_t *dw = reinterpret_cast<uint32_t *>(d + head);
         uint32_t a = w0;
         for (uint32_t j = 0; j < nw; ++j) {
             const uint32_t b = slot[(j + 1) * ET];
             dw[j] = __funnelshift_r(a, b, 8u * head);
             a = b;
         }
-        const uint32_t done = head + 4u * nw;                // a = the slot word holding byte `done - head`... see below
-        for (uint32_t k = done; k < local; ++k) o[k] = (char)(slot[(k >> 2) * ET] >> (8u * (k & 3u)));
+        const uint32_t done = head + 4u * nw;
+        for (uint32_t k = done; k < local; ++k) d[k] = (char)(slot[(k >> 2) * ET] >> (8u * (k & 3u)));
+    };
+    // emit5: the entry array is dead (every walk ended before the scan's barriers) and holds the band's image when no
+    // slot overflowed (<= 84 bytes a thread) and the image fits its 24*w bytes (narrow bands)
+    if (V5 && !__syncthreads_or(ovf) && band_total <= 24u * (uint32_t)w) {
+        char *img = reinterpret_cast<char *>(s_sorted);
+        slot_out(img + at);
+        __syncthreads();
+        const uint32_t n16 = band_total >> 4;
+        const uint4 *s16 = reinterpret_cast<const uint4 *>(img);
+        uint4 *d16 = reinterpret_cast<uint4 *>(band_out);
+        for (uint32_t j = tid; j < n16; j += ET) d16[j] = s16[j];
+        const uint32_t t = (n16 << 4) + (uint32_t)tid;
+        if (t < band_total) band_out[t] = img[t];
+    } else if (!ovf) {
+        slot_out(o);
     } else {                                                 // v1's write walk for this thread's range
         walk_runs(s_sorted, lo, hi, n, [&](uint32_t c, uint32_t bits, uint32_t gap, uint32_t len, bool first) {
             if (first) { if (c != minc) *o++ = '$'; *o++ = '#'; o = put_num4(o, c); }
@@ -906,6 +973,8 @@ sixel_emit1b_kernel(EmitGeom G, SixelWork W) {
             o = put_rle(o, len, (char)('?' + bits));
         });
     }
+    EMIT_CLK();                                              // copy-out
+    EMIT_CLK_END(V5 ? 1 : 0);
 }
 
 // per frame: header length, band offsets (exclusive, in place), frame size
@@ -1023,7 +1092,7 @@ static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 struct SixelPlan {
     SixelWork W;
     bool emit_v1, dither_v1;
-    int emit_mode;                            // 1: v1 (scratch arena + compaction), 2: emit2, 3: emit3 (default)
+    int emit_mode;                            // 1: v1, 4: v1b, 5: emit5 (scratch arena + compaction), 2: emit2, 3: emit3
     EmitGeom G;
     size_t emit_smem, o_d2_bnd, o_d2_prog;
     long long npix;
@@ -1053,18 +1122,19 @@ static int sixel_plan(b200timg_ctx *ctx, int w, int h, int n_frames, bool reserv
     // worst case of one band: <= 6 entries per column, <= 7 bytes each ("!nnnn?" + char), "$#ccc" per colour
     W.band_cap = align_up((size_t)w * 42 + 256 * 5 + 16, 256);
     const size_t o_scr = off;
-    // three emitters (B200TIMG_EMIT=1|2|3): v1 (the default up to 4095 px: per-band sizes into a scratch arena + compaction
-    // kernel), emit2 (sixel_emit.cu: single pass, any width -- what wider frames get) and emit3 (v1's sort + entry-parallel
-    // formatting + look-back placement; slower than v1 on C2 frames, kept for A/B runs only).
+    // the emitters (B200TIMG_EMIT=1..5): v1, v1b (4) and emit5 (5, the default up to 4095 px) write per-band bytes into a
+    // scratch arena for the compaction kernel; emit2 (sixel_emit.cu: single pass, any width -- what wider frames get) and
+    // emit3 (v1's sort + entry-parallel formatting + look-back placement; slower than v1 on C2 frames) place their own.
+    // Every mode but the default is kept for A/B runs.
     {
         const bool v1_fits = w <= 4095 && sizeof(uint32_t) * (size_t)6 * w <= (size_t)(227 - 36) * 1024;
         const bool v1b_fits = w <= 4095 && sizeof(uint32_t) * (size_t)6 * w <= (size_t)(227 - 47) * 1024;
-        int mode = v1b_fits ? 4 : v1_fits ? 1 : 2;           // 4 = v1b: v1 with the single formatting walk
+        int mode = v1b_fits ? 5 : v1_fits ? 1 : 2;           // 5 = emit5 (v1b with staged rows and a coalesced copy-out)
         if (getenv("B200TIMG_EMIT_V2")) mode = 2;
         if (const char *e = getenv("B200TIMG_EMIT")) mode = atoi(e);
-        if (mode < 1 || mode > 4 || (mode == 1 && !v1_fits) || (mode == 4 && !v1b_fits)) mode = 2;
+        if (mode < 1 || mode > 5 || (mode == 1 && !v1_fits) || (mode >= 4 && !v1b_fits)) mode = 2;
         S->emit_mode = mode;
-        S->emit_v1 = mode == 1 || mode == 4;
+        S->emit_v1 = mode == 1 || mode >= 4;
     }
     if (S->emit_v1) off += W.band_cap * W.nbands * n_frames;
     S->dither_v1 = getenv("B200TIMG_DITHER_V1") != nullptr;      // round-1 ditherer, kept for A/B runs
@@ -1091,7 +1161,8 @@ static int sixel_plan(b200timg_ctx *ctx, int w, int h, int n_frames, bool reserv
     if (!ctx->sixel_attrs_set) {                         // function attributes are per device, i.e. per context
         B2_CUDA(ctx, cudaFuncSetAttribute(sixel_palette_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 65536));
         B2_CUDA(ctx, cudaFuncSetAttribute(sixel_emit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit));
-        B2_CUDA(ctx, cudaFuncSetAttribute(sixel_emit1b_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (227 - 47) * 1024));
+        B2_CUDA(ctx, cudaFuncSetAttribute(sixel_emit1b_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (227 - 47) * 1024));
+        B2_CUDA(ctx, cudaFuncSetAttribute(sixel_emit1b_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (227 - 47) * 1024));
         B2_CUDA(ctx, cudaFuncSetAttribute(sixel_dither_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 32768 + DW_MAX * DWARP_SMEM));
         // unconditionally: which variant a frame takes depends on ITS size, not on the first frame this context saw
         B2_CUDA(ctx, cudaFuncSetAttribute(sixel_palette_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
@@ -1143,8 +1214,9 @@ int launch_sixel_front(b200timg_ctx *ctx, const uint8_t *d_fb, int w, int h, int
         B2_LAUNCH_CHECK(ctx);
     }
     if (S.emit_v1) {
-        B2_KERNEL(ctx, "sixel_emit_kernel");
-        if (S.emit_mode == 4) sixel_emit1b_kernel<<<dim3(W.nbands, n), ET, S.emit_smem, ctx->stream>>>(S.G, W);
+        B2_KERNEL(ctx, S.emit_mode == 5 ? "sixel_emit5_kernel" : "sixel_emit_kernel");
+        if (S.emit_mode == 5) sixel_emit1b_kernel<true><<<dim3(W.nbands, n), ET, S.emit_smem, ctx->stream>>>(S.G, W);
+        else if (S.emit_mode == 4) sixel_emit1b_kernel<false><<<dim3(W.nbands, n), ET, S.emit_smem, ctx->stream>>>(S.G, W);
         else sixel_emit_kernel<<<dim3(W.nbands, n), ET, S.emit_smem, ctx->stream>>>(S.G, W);
         B2_LAUNCH_CHECK(ctx);
     }
@@ -1199,3 +1271,15 @@ int sixel_debug_fetch(b200timg_ctx *ctx, uint32_t *h_palette, uint32_t *h_counts
 }
 
 }  // namespace b200timg
+
+#ifdef B200TIMG_EMIT_CLOCKS
+// instrumented builds only: the summed phase clocks [2][8] since the last call (then cleared); 0 or -3 (CUDA error)
+extern "C" int b200timg_emit_clocks(unsigned long long *out) {
+    using b200timg::g_emit_clocks;
+    static const unsigned long long zero[2][b200timg::EMIT_CLK_PHASES] = {};
+    if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpyFromSymbol(out, g_emit_clocks, sizeof zero) != cudaSuccess ||
+        cudaMemcpyToSymbol(g_emit_clocks, zero, sizeof zero) != cudaSuccess)
+        return -3;
+    return 0;
+}
+#endif
