@@ -335,8 +335,24 @@ int b200timg_png_batch_dev(b200timg_ctx *ctx, const uint8_t *d_frames, int w, in
 #define B200TIMG_KITTY      1
 #define B200TIMG_ITERM2     2
 #define B200TIMG_KITTY_TMUX 4   /* KittyGraphicsCanvas with tmux_passthrough_needed (3 is not a protocol) */
+/* B200TIMG_DEFLATE, OR'ed into protocol (any of the three): the PNG's zlib stream is compressed, as timg does for
+ * --compress levels 1-9 (DisplayOptions::compress_pixel_level > 0); level 0 is the stored path above.  All levels
+ * 1-9 map to this library's one compressor (libdeflate's per-level trade-offs are not reproduced): per 65535-byte
+ * segment of the scanline stream, a greedy LZ77 parse (matches of 4 to 258 bytes, up to 32768 bytes back, into the
+ * previous segment too) and one dynamic-Huffman block, or the stored block where that is not at least 2 bytes
+ * smaller.  A frame's PNG is therefore never longer than b200timg_png_size().  The output is deterministic: a frame's
+ * bytes depend on that frame only (not on its place in the batch, the batch size or the variant called).  libdeflate
+ * is not in the reference's tree, so the deflate bytes are not the reference's: they decode to the same pixels, and
+ * every byte around them (PNG chunks and CRCs, base64, chunking, headers, placeholders) is what the reference's own
+ * code writes around this stream.
+ * Sizes depend on the data: b200timg_graphics_size with the bit set returns the stored size, an UPPER BOUND.  The _dev
+ * variant computes d_offsets on the device (exact) and follows the OUTPUT CAPACITY CONTRACT.  The host variant reads
+ * the offsets back chunk by chunk; on B200TIMG_ENOSPC offsets[] is complete (offsets[n_frames] = the bytes needed) and
+ * nothing is written at or beyond out_cap.  Any other bit, and 3 | B200TIMG_DEFLATE, is B200TIMG_EINVAL.
+ * b200timg_png_encode and b200timg_png_batch_dev keep stored blocks. */
+#define B200TIMG_DEFLATE    8
 typedef struct {
-    int protocol;               /* B200TIMG_KITTY, B200TIMG_ITERM2 or B200TIMG_KITTY_TMUX */
+    int protocol;               /* B200TIMG_KITTY, B200TIMG_ITERM2 or B200TIMG_KITTY_TMUX, optionally | B200TIMG_DEFLATE */
     int rgb24;                  /* DisplayOptions::local_alpha_handling: PNG colour type 2, else RGBA (type 6) */
     const uint32_t *ids;        /* kitty (either form): n_frames image ids (HOST pointer), the i= of each frame;
                                    ignored for iTerm2 */

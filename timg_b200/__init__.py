@@ -32,6 +32,7 @@ def yuv_frame_bytes(fmt, w, h):
 
 
 KITTY, ITERM2, KITTY_TMUX = 1, 2, 4
+DEFLATE = 8      # OR'ed into a protocol: compressed PNGs (timg's --compress 1-9); sizes are then upper bounds
 
 u8p = C.POINTER(C.c_uint8)
 u64p = C.POINTER(C.c_uint64)

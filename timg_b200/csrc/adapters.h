@@ -222,7 +222,8 @@ private:
 // from one b200timg_graphics_batch call with n_frames = 1: the frame is shown as it is (source = output geometry, so
 // the scaler is a copy) and not composed, as the reference's canvases do (src/iterm2-canvas.cc:55-75,
 // src/kitty-canvas.cc:178-231).  Exactly the framed bytes come back, written straight after the prefix.  The PNG
-// itself uses stored deflate blocks, so the base64 payload is larger than libdeflate's but decodes to the same pixels.
+// uses stored deflate blocks, or with deflate (timg's --compress > 0) this library's compressor; either decodes to the
+// same pixels as libdeflate's.  n is b200timg_graphics_size, the exact size or, compressed, an upper bound.
 inline char *B200AppendGraphics(const Framebuffer &fb, const b200timg_graphics &g, char *pos, size_t n) {
     b200timg_batch b{};
     b.n_frames = 1;
@@ -233,12 +234,14 @@ inline char *B200AppendGraphics(const Framebuffer &fb, const b200timg_graphics &
     std::lock_guard<std::mutex> l(B200Context::Lock());
     B200Context::Check(b200timg_graphics_batch(B200Context::Get(), &b, &g, (const uint8_t *)fb.begin(), pos, n, offsets),
                        "graphics_batch");
-    return pos + n;
+    return pos + offsets[1];
 }
 
 class B200ITerm2Canvas final : public TerminalCanvas {
 public:
-    B200ITerm2Canvas(BufferedWriteSequencer *ws, const DisplayOptions &opts) : TerminalCanvas(ws), options_(opts) {}
+    // deflate: compressed PNGs (DisplayOptions::compress_pixel_level > 0); false keeps stored blocks
+    B200ITerm2Canvas(BufferedWriteSequencer *ws, const DisplayOptions &opts, bool deflate = false)
+        : TerminalCanvas(ws), options_(opts), deflate_(deflate) {}
     int cell_height_for_pixels(int pixels) const final {                                // src/iterm2-canvas.cc:91-95
         assert(pixels <= 0);
         return -((-pixels + options_.cell_y_px - 1) / options_.cell_y_px);
@@ -247,7 +250,7 @@ public:
         if (dy < 0) MoveCursorDY(cell_height_for_pixels(dy));
         MoveCursorDX(x / options_.cell_x_px);
         b200timg_graphics g{};
-        g.protocol = B200TIMG_ITERM2;
+        g.protocol = B200TIMG_ITERM2 | (deflate_ ? B200TIMG_DEFLATE : 0);
         g.rgb24 = options_.local_alpha_handling ? 1 : 0;
         const size_t n = b200timg_graphics_size(&g, fb.width(), fb.height(), 0);
         char *buffer = new char[n + 4096];
@@ -257,15 +260,18 @@ public:
 
 private:
     const DisplayOptions &options_;
+    const bool deflate_;
 };
 
 class B200KittyCanvas final : public TerminalCanvas {
 public:
-    B200KittyCanvas(BufferedWriteSequencer *ws, const DisplayOptions &opts) : B200KittyCanvas(ws, false, opts) {}
+    B200KittyCanvas(BufferedWriteSequencer *ws, const DisplayOptions &opts, bool deflate = false)
+        : B200KittyCanvas(ws, false, opts, deflate) {}
     // tmux_passthrough_needed: the tmux form (src/kitty-canvas.cc:113-124), which timg picks when the terminal
     // query reports tmux (PresentImages' present.tmux_workaround)
-    B200KittyCanvas(BufferedWriteSequencer *ws, bool tmux_passthrough_needed, const DisplayOptions &opts)
-        : TerminalCanvas(ws), options_(opts), tmux_(tmux_passthrough_needed) {
+    // deflate: compressed PNGs (DisplayOptions::compress_pixel_level > 0); false keeps stored blocks
+    B200KittyCanvas(BufferedWriteSequencer *ws, bool tmux_passthrough_needed, const DisplayOptions &opts, bool deflate = false)
+        : TerminalCanvas(ws), options_(opts), tmux_(tmux_passthrough_needed), deflate_(deflate) {
         if (tmux_) EnableTmuxPassthrough();
     }
     int cell_height_for_pixels(int pixels) const final {                                // src/kitty-canvas.cc:248-252
@@ -283,7 +289,7 @@ public:
         case SeqType::ControlWrite: break;
         }
         b200timg_graphics g{};
-        g.protocol = tmux_ ? B200TIMG_KITTY_TMUX : B200TIMG_KITTY;
+        g.protocol = (tmux_ ? B200TIMG_KITTY_TMUX : B200TIMG_KITTY) | (deflate_ ? B200TIMG_DEFLATE : 0);
         g.rgb24 = options_.local_alpha_handling ? 1 : 0;
         g.ids = &id;
         g.cell_x_px = options_.cell_x_px;                                               // .cc:174-176
@@ -312,7 +318,7 @@ private:
         return kStart + counter;
     }
     const DisplayOptions &options_;
-    const bool tmux_;
+    const bool tmux_, deflate_;
     uint32_t animation_id_ = 0;
     uint8_t flip_buffer_ = 0;
 };

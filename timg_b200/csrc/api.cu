@@ -76,6 +76,7 @@ void b200timg_ctx_destroy(b200timg_ctx *ctx) {
     ctx->tables.release(); ctx->sixel_work.release(); ctx->misc.release(); ctx->scale_list.release(); ctx->scale_tmp.release(); ctx->tri_tables.release();
     ctx->pinned.release(); ctx->pinned_io.release();
     ctx->png_sums.release(); ctx->gfx_ids.release();
+    ctx->dfl_raw.release(); ctx->dfl_scratch.release(); ctx->dfl_meta.release(); ctx->dfl_tokens.release(); ctx->dfl_png.release();
     for (int i = 0; i < 4; ++i) { ctx->gfx_stage[i].release(); if (ctx->ev_gfx[i]) cudaEventDestroy(ctx->ev_gfx[i]); }
     for (int i = 0; i < 2; ++i) { ctx->pipe_in[i].release(); ctx->pipe_out[i].release(); }
     if (ctx->parts_ready) {
@@ -509,10 +510,11 @@ int b200timg_sixel_batch_dev(b200timg_ctx *ctx, const b200timg_batch *b, const u
 // ---- kitty / iTerm2 batches ------------------------------------------------------------------
 static int validate_graphics(b200timg_ctx *ctx, const b200timg_batch *b, const b200timg_graphics *g) {
     if (!g) return ctx->fail(B200TIMG_EINVAL, "graphics: null protocol description");
-    if (g->protocol != B200TIMG_KITTY && g->protocol != B200TIMG_ITERM2 && g->protocol != B200TIMG_KITTY_TMUX)
+    const int protocol = g->protocol & ~B200TIMG_DEFLATE;
+    if (protocol != B200TIMG_KITTY && protocol != B200TIMG_ITERM2 && protocol != B200TIMG_KITTY_TMUX)
         return ctx->fail(B200TIMG_EINVAL, "graphics: unknown protocol %d", g->protocol);
-    if (g->protocol != B200TIMG_ITERM2 && !g->ids) return ctx->fail(B200TIMG_EINVAL, "graphics: kitty needs one image id per frame (ids is NULL)");
-    if (g->protocol == B200TIMG_KITTY_TMUX && (g->cell_x_px <= 0 || g->cell_y_px <= 0 || g->indent_cells < 0))
+    if (protocol != B200TIMG_ITERM2 && !g->ids) return ctx->fail(B200TIMG_EINVAL, "graphics: kitty needs one image id per frame (ids is NULL)");
+    if (protocol == B200TIMG_KITTY_TMUX && (g->cell_x_px <= 0 || g->cell_y_px <= 0 || g->indent_cells < 0))
         return ctx->fail(B200TIMG_EINVAL, "graphics: tmux placeholders need a positive cell size and indent >= 0 (cell %dx%d, indent %d)",
                          g->cell_x_px, g->cell_y_px, g->indent_cells);
     if (b->animation != 0) return ctx->fail(B200TIMG_EINVAL, "graphics: kitty / iTerm2 frames have no delta encoding (animation must be 0)");
@@ -524,7 +526,7 @@ static int validate_graphics(b200timg_ctx *ctx, const b200timg_batch *b, const b
 // offsets[0..n]: the running sum of the frame sizes
 static void graphics_offsets(const b200timg_batch *b, const b200timg_graphics *g, uint64_t *offsets) {
     offsets[0] = 0;
-    const bool kitty = g->protocol != B200TIMG_ITERM2;
+    const bool kitty = (g->protocol & ~B200TIMG_DEFLATE) != B200TIMG_ITERM2;
     for (int f = 0; f < b->n_frames; ++f) offsets[f + 1] = offsets[f] + b200timg_graphics_size(g, b->out_w, b->out_h, kitty ? g->ids[f] : 0);
 }
 
@@ -535,7 +537,8 @@ int b200timg_graphics_batch_dev(b200timg_ctx *ctx, const b200timg_batch *b, cons
     if (!d_src || !d_out || !d_offsets) return ctx->fail(B200TIMG_EINVAL, "batch: null pointer");
     B2_TRY(validate_graphics(ctx, b, g));
     const int n = b->n_frames;
-    const bool kitty = g->protocol != B200TIMG_ITERM2;           // either kitty form: image ids go up too
+    const bool kitty = (g->protocol & ~B200TIMG_DEFLATE) != B200TIMG_ITERM2;   // either kitty form: image ids go up too
+    const bool deflate = (g->protocol & B200TIMG_DEFLATE) != 0;              // sizes known only on the device
     // offsets (and kitty's ids) are computed here and go up from a pinned slot; the slot is only rewritten once the
     // copy that last read it has run, which never waits unless four batches are queued behind each other
     const int slot = ctx->gfx_slot;
@@ -545,8 +548,10 @@ int b200timg_graphics_batch_dev(b200timg_ctx *ctx, const b200timg_batch *b, cons
     const size_t off_bytes = (size_t)(n + 1) * sizeof(uint64_t), id_bytes = kitty ? (size_t)n * sizeof(uint32_t) : 0;
     B2_CUDA(ctx, ctx->gfx_stage[slot].reserve(off_bytes + id_bytes));
     uint64_t *h_offs = ctx->gfx_stage[slot].as<uint64_t>();
-    graphics_offsets(b, g, h_offs);
-    B2_CUDA(ctx, cudaMemcpyAsync(d_offsets, h_offs, off_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    if (!deflate) {
+        graphics_offsets(b, g, h_offs);
+        B2_CUDA(ctx, cudaMemcpyAsync(d_offsets, h_offs, off_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    }
     if (kitty) {
         B2_CUDA(ctx, ctx->gfx_ids.reserve(id_bytes));
         memcpy(h_offs + n + 1, g->ids, id_bytes);
@@ -601,8 +606,12 @@ static int batch_host_impl(b200timg_ctx *ctx, const b200timg_batch *b, const uin
     B2_TRY(validate_batch(ctx, b));
     if (!src || !out || !offsets) return ctx->fail(B200TIMG_EINVAL, "batch: null pointer");
     const bool sixel = enc == Encoder::sixel, graphics = enc == Encoder::graphics;
-    if (graphics) {                                            // every size is known now: nothing runs if they do not fit
-        B2_TRY(validate_graphics(ctx, b, gfx));
+    // stored-block graphics: every size is known before the call; with B200TIMG_DEFLATE they are read back per chunk,
+    // and running short of out_cap still completes offsets[] (nothing more is downloaded)
+    const bool deflate = graphics && gfx && (gfx->protocol & B200TIMG_DEFLATE), sized = graphics && !deflate;
+    bool short_of_space = false;
+    if (graphics) B2_TRY(validate_graphics(ctx, b, gfx));
+    if (sized) {                                               // every size is known now: nothing runs if they do not fit
         graphics_offsets(b, gfx, offsets);
         if (offsets[b->n_frames] > out_cap)
             return ctx->fail(B200TIMG_ENOSPC, "batch: need %llu bytes (have %zu)", (unsigned long long)offsets[b->n_frames], out_cap);
@@ -635,7 +644,7 @@ static int batch_host_impl(b200timg_ctx *ctx, const b200timg_batch *b, const uin
     B2_TRY(upload_chunk(0));
     if (n_chunks > 1) B2_TRY(upload_chunk(1));
     size_t base_bytes = 0;
-    if (!graphics) offsets[0] = 0;
+    if (!sized) offsets[0] = 0;
     for (int k = 0; k < n_chunks; ++k) {
         const int i = k & 1, f0 = k * chunk, nf = std::min(chunk, b->n_frames - f0);
         const int halo = (anim && k > 0) ? 1 : 0;             // the sub-batch then starts one frame early
@@ -652,7 +661,7 @@ static int batch_host_impl(b200timg_ctx *ctx, const b200timg_batch *b, const uin
             sub_gfx.protocol = gfx->protocol;
             sub_gfx.rgb24 = gfx->rgb24;
             sub_gfx.ids = gfx->ids ? gfx->ids + f0 : nullptr;
-            if (gfx->protocol == B200TIMG_KITTY_TMUX) {
+            if ((gfx->protocol & ~B200TIMG_DEFLATE) == B200TIMG_KITTY_TMUX) {
                 sub_gfx.cell_x_px = gfx->cell_x_px;
                 sub_gfx.cell_y_px = gfx->cell_y_px;
                 sub_gfx.indent_cells = gfx->indent_cells;
@@ -670,13 +679,18 @@ static int batch_host_impl(b200timg_ctx *ctx, const b200timg_batch *b, const uin
             B2_TRY(upload_chunk(k + 2));
         }
         size_t total = 0;
-        if (graphics) total = (size_t)(offsets[f0 + nf] - offsets[f0]);           // known before the call
+        if (sized) total = (size_t)(offsets[f0 + nf] - offsets[f0]);              // known before the call
         else {
             B2_CUDA(ctx, cudaMemcpyAsync(h_offs, ctx->offsets.p, (size_t)(nf + halo + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
             B2_CUDA(ctx, cudaEventRecord(ctx->ev_prep, ctx->stream));
             B2_CUDA(ctx, cudaEventSynchronize(ctx->ev_prep));                      // sizes of this chunk are on the host
             total = (size_t)h_offs[nf + halo];                                     // a halo frame contributes no bytes
             for (int j = 1; j <= nf; ++j) offsets[f0 + j] = base_bytes + h_offs[j + halo];
+        }
+        if (deflate && (short_of_space || base_bytes + total > out_cap)) {
+            short_of_space = true;
+            base_bytes += total;
+            continue;
         }
         if (base_bytes + total > out_cap) {
             return ctx->fail(B200TIMG_ENOSPC, "batch: need more than %zu bytes (have %zu)", base_bytes + total, out_cap);
@@ -689,6 +703,10 @@ static int batch_host_impl(b200timg_ctx *ctx, const b200timg_batch *b, const uin
         base_bytes += total;
     }
     B2_CUDA(ctx, cudaStreamSynchronize(ctx->d2h_stream));
+    if (short_of_space) {
+        B2_TRY(sync(ctx));
+        return ctx->fail(B200TIMG_ENOSPC, "batch: need %zu bytes (have %zu)", base_bytes, out_cap);
+    }
     return sync(ctx);
 }
 

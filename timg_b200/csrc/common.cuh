@@ -91,6 +91,9 @@ struct b200timg_ctx {
     b200timg::HostBuf pinned;      // staging for sizes / offsets
     b200timg::DevBuf png_sums;     // per frame: Adler-32 and IDAT CRC-32 of the PNG (png.cu)
     b200timg::DevBuf gfx_ids;      // kitty image ids of a graphics batch
+    // B200TIMG_DEFLATE (deflate.cu, png.cu): scanline streams, per-segment blocks and their records, the parse's
+    // tokens, the PNG files
+    b200timg::DevBuf dfl_raw, dfl_scratch, dfl_meta, dfl_tokens, dfl_png;
     // offsets + ids of a graphics batch go up from here; a slot is reused once its copy has run (ev_gfx)
     b200timg::HostBuf gfx_stage[4];
     cudaEvent_t ev_gfx[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -250,9 +253,19 @@ int launch_sixel(b200timg_ctx *ctx, const uint8_t *d_fb, int w, int h, int n_fra
                  size_t out_cap, uint64_t *d_offsets, int phases);
 int launch_sixel_front(b200timg_ctx *ctx, const uint8_t *d_fb, int w, int h, int n_total, int f0, int n, bool reserve);
 int launch_sixel_back(b200timg_ctx *ctx, int w, int h, int n_frames, char *d_out, size_t out_cap, uint64_t *d_offsets, int phases);
-// kitty / iTerm2 text of n composed frames at d_out + d_offsets[f] (png.cu); d_ids: kitty image ids
+// kitty / iTerm2 text of n composed frames at d_out + d_offsets[f] (png.cu); d_ids: kitty image ids.  With
+// B200TIMG_DEFLATE the offsets are computed on the device and written to d_offsets.
 int launch_graphics(b200timg_ctx *ctx, const uint8_t *d_frames, int w, int h, int n_frames, const b200timg_graphics &gr,
-                    const uint32_t *d_ids, const uint64_t *d_offsets, char *d_out, size_t out_cap);
+                    const uint32_t *d_ids, uint64_t *d_offsets, char *d_out, size_t out_cap);
+// deflate.cu: the dynamic-Huffman blocks of every 65535-byte segment of n scanline streams (frame f at
+// d_raw + f * raw_stride) into DFL_SLOT-byte scratch slots, then every block at its bit offset in its frame's PNG slot
+struct DeflateSeg { uint32_t bits, stored; };     // the block's size in bits (dynamic) or stored = 1
+constexpr long long DFL_SLOT = 65552;             // >= the largest dynamic block kept (65538 bytes) + one zero word
+int launch_deflate(b200timg_ctx *ctx, const uint8_t *d_raw, long long raw_stride, int raw_len, int n_frames, int nseg,
+                   uint8_t *d_scratch, DeflateSeg *d_info);
+int launch_deflate_pack(b200timg_ctx *ctx, const uint8_t *d_raw, long long raw_stride, int raw_len, int n_frames, int nseg,
+                        const uint8_t *d_scratch, const DeflateSeg *d_info, const unsigned long long *d_start, uint8_t *d_png,
+                        long long png_stride, int zoff);
 int sixel_debug_fetch(b200timg_ctx *ctx, uint32_t *h_palette, uint32_t *h_counts, uint8_t *h_index, size_t index_bytes);
 
 }  // namespace b200timg

@@ -213,7 +213,8 @@ png_seal_kernel(PngGeom g, int nseg_crc, int nseg_raw, const SegSum *__restrict_
 
 // The checksum pass shared by the PNG files and the framed batches: segment sums from the frames, then two words per
 // frame in ctx->png_sums (and, when png is given, the checksum fields of those files).
-static int launch_png_sums(b200timg_ctx *ctx, const uint8_t *d_frames, const PngGeom &g, int n_frames, uint8_t *d_png);
+static int launch_png_sums(b200timg_ctx *ctx, const uint8_t *d_frames, const PngGeom &g, int n_frames, uint8_t *d_png,
+                           bool with_crc = true);
 
 // ---- base64 (src/timg-base64.h:28-53): n bytes -> 4*ceil(n/3) characters, per frame ---------------------
 __global__ void __launch_bounds__(256)
@@ -240,8 +241,9 @@ static unsigned png_grid(b200timg_ctx *ctx, long long items, int threads) {
     return (unsigned)(b < 1 ? 1 : b);
 }
 
-static int launch_png_sums(b200timg_ctx *ctx, const uint8_t *d_frames, const PngGeom &g, int n_frames, uint8_t *d_png) {
-    const int nseg_crc = (int)((4 + g.zlib_len + PNG_SEG - 1) / PNG_SEG), nseg_raw = (int)((g.raw_len + PNG_SEG - 1) / PNG_SEG);
+static int launch_png_sums(b200timg_ctx *ctx, const uint8_t *d_frames, const PngGeom &g, int n_frames, uint8_t *d_png,
+                           bool with_crc) {
+    const int nseg_crc = with_crc ? (int)((4 + g.zlib_len + PNG_SEG - 1) / PNG_SEG) : 0, nseg_raw = (int)((g.raw_len + PNG_SEG - 1) / PNG_SEG);
     B2_CUDA(ctx, ctx->cells.reserve(sizeof(SegSum) * (size_t)(nseg_crc + nseg_raw) * n_frames));
     B2_CUDA(ctx, ctx->png_sums.reserve(2 * sizeof(uint32_t) * (size_t)n_frames));
     SegSum *seg = ctx->cells.as<SegSum>();
@@ -288,8 +290,8 @@ struct GfxSpec {
 };
 // the placeholder fields are read for the tmux form only
 static GfxSpec gfx_spec(const b200timg_graphics &gr, const PngGeom &g) {
-    GfxSpec s{gr.protocol, g.w, g.h, g.png_len, (g.png_len + GFX_BYTES - 1) / GFX_BYTES, 0, 0, 0};
-    if (gr.protocol == B200TIMG_KITTY_TMUX) {
+    GfxSpec s{gr.protocol & ~B200TIMG_DEFLATE, g.w, g.h, g.png_len, (g.png_len + GFX_BYTES - 1) / GFX_BYTES, 0, 0, 0};
+    if (s.protocol == B200TIMG_KITTY_TMUX) {
         s.cols = g.w / gr.cell_x_px;
         s.rows = (g.h + gr.cell_y_px - 1) / gr.cell_y_px;
         s.indent = gr.indent_cells;
@@ -462,7 +464,7 @@ __host__ __device__ inline long long grid_row_base(const GfxSpec &s, uint32_t id
 
 // A closed formula: every part that depends on the id (its digits, the colour's digits, the msb diacritic) is largest
 // at id = 0xffffffff, so the size at that id bounds the size at any id of the same geometry.
-static size_t gfx_frame_size(const GfxSpec &s, uint32_t id) {
+__host__ __device__ inline size_t gfx_frame_size(const GfxSpec &s, uint32_t id) {
     long long n = gfx_text_len(s, id);
     if (s.protocol == B200TIMG_KITTY_TMUX) n += (long long)s.rows * grid_row_base(s, id) + (long long)s.cols * diac_prefix(s.rows);
     return (size_t)n;
@@ -470,6 +472,14 @@ static size_t gfx_frame_size(const GfxSpec &s, uint32_t id) {
 
 __device__ __forceinline__ char b64_char(uint32_t v) {
     return (char)(v < 26 ? 'A' + v : v < 52 ? 'a' + (v - 26) : v < 62 ? '0' + (v - 52) : v == 62 ? '+' : '/');
+}
+
+// B200TIMG_DEFLATE: a frame's PNG length (and so its kitty chunks and iTerm2's size=) comes from png_lens on the
+// device; s then describes the stored-size bound
+__host__ __device__ inline GfxSpec frame_spec(const GfxSpec &s, const uint32_t *png_lens, int f) {
+    GfxSpec r = s;
+    if (png_lens) { r.png_len = png_lens[f]; r.tiles = (r.png_len + GFX_BYTES - 1) / GFX_BYTES; }
+    return r;
 }
 
 constexpr int GFX_THREADS = 256;
@@ -486,22 +496,25 @@ __device__ __forceinline__ void copy_out16(char *base, const char *s_txt, int sh
 // One CTA per tile (grid-stride): stage the tile's PNG bytes from the frame, build its text in shared memory at the
 // destination's alignment mod 16, copy it out with 16-byte stores.  A frame that would end beyond out_cap is skipped.
 __global__ void __launch_bounds__(GFX_THREADS)
-graphics_emit_kernel(const uint8_t *__restrict__ frames, PngGeom g, GfxSpec s, int n_frames, const uint32_t *__restrict__ ids,
+graphics_emit_kernel(const uint8_t *__restrict__ frames, PngGeom g, GfxSpec s_max, int n_frames, const uint32_t *__restrict__ ids,
                      const uint32_t *__restrict__ sums, uint32_t ihdr, const uint64_t *__restrict__ offsets, char *__restrict__ out,
-                     unsigned long long out_cap) {
+                     unsigned long long out_cap, const uint8_t *__restrict__ pngs, long long png_stride,
+                     const uint32_t *__restrict__ png_lens) {
     __shared__ uint8_t s_png[GFX_BYTES];
     __shared__ __align__(16) char s_txt[4352];          // 15 (alignment) + header (<= 72) + 4096 + separator (<= 24)
-    const long long total = (long long)n_frames * s.tiles;
+    const long long total = (long long)n_frames * s_max.tiles;
     for (long long t = blockIdx.x; t < total; t += gridDim.x) {
-        const int f = (int)(t / s.tiles);
-        const long long c = t - (long long)f * s.tiles;
-        if (offsets[f + 1] > out_cap) continue;          // the same for every thread of the CTA
+        const int f = (int)(t / s_max.tiles);
+        const long long c = t - (long long)f * s_max.tiles;
+        const GfxSpec s = frame_spec(s_max, png_lens, f);
+        if (c >= s.tiles || offsets[f + 1] > out_cap) continue;          // the same for every thread of the CTA
         const uint32_t id = ids ? ids[f] : 0u;
         const uint8_t *fb = frames + (long long)f * g.w * g.h * 4;
         const uint32_t adler = sums[2 * f], crc = sums[2 * f + 1];
         const long long lo = c * GFX_BYTES;
         const int nb = (int)min((long long)GFX_BYTES, s.png_len - lo);
-        for (int k = threadIdx.x; k < nb; k += GFX_THREADS) s_png[k] = png_byte(fb, g, lo + k, ihdr, crc, adler);
+        for (int k = threadIdx.x; k < nb; k += GFX_THREADS)
+            s_png[k] = pngs ? pngs[f * png_stride + lo + k] : png_byte(fb, g, lo + k, ihdr, crc, adler);
         const int hl = gfx_header(nullptr, s, id), pre = c == 0 ? hl : 0;
         const unsigned long long pos = c == 0 ? 0ull : (unsigned long long)hl + c * (4096ull + gfx_sep(s));
         char *dst = out + offsets[f] + pos;
@@ -536,15 +549,16 @@ graphics_emit_kernel(const uint8_t *__restrict__ frames, PngGeom g, GfxSpec s, i
 // out_cap are skipped, as in graphics_emit_kernel.
 constexpr int GRID_CELLS = 256;
 __global__ void __launch_bounds__(GFX_THREADS)
-graphics_grid_kernel(GfxSpec s, int n_frames, const uint32_t *__restrict__ ids, const uint64_t *__restrict__ offsets,
-                     char *__restrict__ out, unsigned long long out_cap) {
+graphics_grid_kernel(GfxSpec s_all, int n_frames, const uint32_t *__restrict__ ids, const uint64_t *__restrict__ offsets,
+                     char *__restrict__ out, unsigned long long out_cap, const uint32_t *__restrict__ png_lens) {
     __shared__ __align__(16) char s_txt[4096];          // 15 (alignment) + head (<= 32) + 256 placeholders (<= 15 each) + tail (7)
-    const int segs = s.cols > GRID_CELLS ? (s.cols + GRID_CELLS - 1) / GRID_CELLS : 1;
-    const long long per_frame = (long long)s.rows * segs, total = per_frame * n_frames;
+    const int segs = s_all.cols > GRID_CELLS ? (s_all.cols + GRID_CELLS - 1) / GRID_CELLS : 1;
+    const long long per_frame = (long long)s_all.rows * segs, total = per_frame * n_frames;
     for (long long t = blockIdx.x; t < total; t += gridDim.x) {
         const int f = (int)(t / per_frame);
         const long long q = t - (long long)f * per_frame;
         const int r = (int)(q / segs), sg = (int)(q - (long long)r * segs);
+        const GfxSpec s = frame_spec(s_all, png_lens, f);
         if (offsets[f + 1] > out_cap) continue;          // the same for every thread of the CTA
         const uint32_t id = ids[f], msb = id >> 24;
         const int head = grid_row_head(nullptr, s, id);
@@ -575,25 +589,163 @@ graphics_grid_kernel(GfxSpec s, int n_frames, const uint32_t *__restrict__ ids, 
     }
 }
 
-// n composed frames (RGBA8, device) -> their framed kitty / iTerm2 text at d_out + d_offsets[f] (offsets already on
-// the device, computed by the caller from b200timg_graphics_size).
+// ---- B200TIMG_DEFLATE: the PNG of every frame, with a compressed zlib body, in a slot of the stored size ----------------
+// raw_fill_kernel writes the scanline streams, deflate.cu compresses them segment by segment, deflate_layout_kernel
+// places the blocks and sizes the frames, deflate_pack_kernel writes the blocks, png_wrap_kernel everything around them
+// but the IDAT CRC, which png_crc_kernel / png_crc_seal_kernel compute from the file's bytes.
+__global__ void __launch_bounds__(256)
+raw_fill_kernel(const uint8_t *__restrict__ frames, PngGeom g, int n_frames, uint8_t *__restrict__ raw, long long raw_stride) {
+    const long long total = g.raw_len * n_frames;
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
+        const long long f = t / g.raw_len, i = t - f * g.raw_len;
+        raw[f * raw_stride + i] = raw_byte(frames + f * (long long)g.w * g.h * 4, g, i);
+    }
+}
+
+// One CTA: per frame, the bit offset of every block (in order; a stored block's size depends on where it lands), the
+// PNG length and the frame's framed size; then offsets[] as their running sum.
+__global__ void __launch_bounds__(1024)
+deflate_layout_kernel(PngGeom g, GfxSpec s, int n_frames, int nseg, const DeflateSeg *__restrict__ info,
+                      unsigned long long *__restrict__ start, uint32_t *__restrict__ png_lens, const uint32_t *__restrict__ ids,
+                      uint64_t *__restrict__ offsets) {
+    __shared__ unsigned long long part[1024];
+    for (int f = threadIdx.x; f < n_frames; f += blockDim.x) {
+        unsigned long long e = 0;
+        for (int k = 0; k < nseg; ++k) {
+            const long long t = (long long)f * nseg + k;
+            start[t] = e;
+            const DeflateSeg sg = info[t];
+            const long long n = min((long long)65535, g.raw_len - (long long)k * 65535);
+            e = sg.stored ? ((e + 10) & ~7ull) + 32 + 8ull * n : e + sg.bits;
+        }
+        png_lens[f] = (uint32_t)(g.idat_data_off + 2 + (e + 7) / 8 + 4 + 4 + 12);
+        offsets[f + 1] = gfx_frame_size(frame_spec(s, png_lens, f), ids ? ids[f] : 0u);
+    }
+    __syncthreads();
+    const int per = (n_frames + 1023) / 1024, a = min(n_frames, (int)threadIdx.x * per), b = min(n_frames, a + per);
+    unsigned long long sum = 0;
+    for (int f = a; f < b; ++f) sum += offsets[f + 1];
+    part[threadIdx.x] = sum;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        unsigned long long r = 0;
+        for (int i = 0; i < 1024; ++i) { const unsigned long long v = part[i]; part[i] = r; r += v; }
+        offsets[0] = 0;
+    }
+    __syncthreads();
+    unsigned long long r = part[threadIdx.x];
+    for (int f = a; f < b; ++f) { r += offsets[f + 1]; offsets[f + 1] = r; }
+}
+
+// one thread per frame: signature, IHDR, IDAT length and type, zlib header, Adler-32, IEND
+__global__ void png_wrap_kernel(PngGeom g, int n_frames, const uint32_t *__restrict__ png_lens, const uint32_t *__restrict__ sums,
+                                uint32_t ihdr, uint8_t *__restrict__ png, long long png_stride) {
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= n_frames) return;
+    uint8_t *p = png + f * png_stride;
+    PngGeom gf = g;
+    gf.png_len = png_lens[f];
+    gf.zlib_len = gf.png_len - gf.idat_data_off - 16;
+    for (long long o = 0; o < gf.idat_data_off + 2; ++o) p[o] = png_byte(nullptr, gf, o, ihdr, 0, 0);
+    put_be32(p + gf.idat_data_off + gf.zlib_len - 4, sums[2 * f]);
+    for (long long o = gf.png_len - 12; o < gf.png_len; ++o) p[o] = png_byte(nullptr, gf, o, ihdr, 0, 0);
+}
+
+// CRC-32 of PNG_SEG-byte pieces of each file's [type "IDAT" .. end of zlib stream]; pieces past the end are empty
+__global__ void __launch_bounds__(128)
+png_crc_kernel(const uint8_t *__restrict__ png, long long png_stride, const uint32_t *__restrict__ png_lens, int n_frames,
+               int npiece, SegSum *__restrict__ seg) {
+    const long long total = (long long)npiece * n_frames;
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
+        const long long f = t / npiece, s = t - f * npiece;
+        const long long region = (long long)png_lens[f] - 53;                 // "IDAT" + zlib stream
+        const long long lo = s * PNG_SEG, hi = min(lo + PNG_SEG, region);
+        const uint8_t *p = png + f * png_stride + 37;
+        uint32_t c = 0xffffffffu;
+        for (long long i = lo; i < hi; ++i) c = crc_byte(c, p[i]);
+        seg[t] = SegSum{c ^ 0xffffffffu, 0, 0};
+    }
+}
+
+__global__ void png_crc_seal_kernel(const SegSum *__restrict__ seg, int n_frames, int npiece, const uint32_t *__restrict__ png_lens,
+                                    uint32_t xn_full, uint8_t *__restrict__ png, long long png_stride) {
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= n_frames) return;
+    const long long region = (long long)png_lens[f] - 53;
+    uint32_t crc = 0;
+    for (int i = 0; i < npiece && (long long)i * PNG_SEG < region; ++i) {
+        const long long len = min((long long)PNG_SEG, region - (long long)i * PNG_SEG);
+        const uint32_t xn = len == PNG_SEG ? xn_full : x8nmodp((unsigned long long)len);
+        crc = i == 0 ? seg[(long long)f * npiece].crc : (multmodp(xn, crc) ^ seg[(long long)f * npiece + i].crc);
+    }
+    put_be32(png + f * png_stride + 37 + region, crc);
+}
+
+// The PNG files of a B200TIMG_DEFLATE batch at ctx->dfl_png (stride png_stride), their lengths at *png_lens and the
+// frames' offsets at d_offsets.
+static int launch_png_deflate(b200timg_ctx *ctx, const uint8_t *d_frames, const PngGeom &g, int n_frames, const GfxSpec &s,
+                              const uint32_t *d_ids, uint64_t *d_offsets, long long png_stride, uint32_t **png_lens) {
+    const int nseg = (int)g.nblocks, npiece = (int)((4 + g.zlib_len + PNG_SEG - 1) / PNG_SEG);
+    const long long raw_stride = (g.raw_len + 15) / 16 * 16, segs = (long long)nseg * n_frames;
+    B2_CUDA(ctx, ctx->dfl_raw.reserve((size_t)(raw_stride * n_frames)));
+    B2_CUDA(ctx, ctx->dfl_scratch.reserve((size_t)(segs * DFL_SLOT)));
+    B2_CUDA(ctx, ctx->dfl_png.reserve((size_t)(png_stride * n_frames)));
+    const size_t info_b = sizeof(DeflateSeg) * segs, start_b = sizeof(unsigned long long) * segs, lens_b = (sizeof(uint32_t) * n_frames + 7) / 8 * 8;
+    B2_CUDA(ctx, ctx->dfl_meta.reserve(info_b + start_b + lens_b + sizeof(SegSum) * (size_t)npiece * n_frames));
+    DeflateSeg *info = ctx->dfl_meta.as<DeflateSeg>();
+    unsigned long long *start = reinterpret_cast<unsigned long long *>(ctx->dfl_meta.as<uint8_t>() + info_b);
+    uint32_t *lens = reinterpret_cast<uint32_t *>(ctx->dfl_meta.as<uint8_t>() + info_b + start_b);
+    SegSum *pieces = reinterpret_cast<SegSum *>(ctx->dfl_meta.as<uint8_t>() + info_b + start_b + lens_b);
+    uint8_t *raw = ctx->dfl_raw.as<uint8_t>(), *png = ctx->dfl_png.as<uint8_t>();
+    B2_KERNEL(ctx, "raw_fill_kernel");
+    raw_fill_kernel<<<png_grid(ctx, g.raw_len * n_frames, 256), 256, 0, ctx->stream>>>(d_frames, g, n_frames, raw, raw_stride);
+    B2_LAUNCH_CHECK(ctx);
+    B2_TRY(launch_png_sums(ctx, d_frames, g, n_frames, nullptr, false));          // Adler-32 only
+    B2_TRY(launch_deflate(ctx, raw, raw_stride, (int)g.raw_len, n_frames, nseg, ctx->dfl_scratch.as<uint8_t>(), info));
+    B2_KERNEL(ctx, "deflate_layout_kernel");
+    deflate_layout_kernel<<<1, 1024, 0, ctx->stream>>>(g, s, n_frames, nseg, info, start, lens, d_ids, d_offsets);
+    B2_LAUNCH_CHECK(ctx);
+    B2_CUDA(ctx, cudaMemsetAsync(png, 0, (size_t)(png_stride * n_frames), ctx->stream));
+    B2_TRY(launch_deflate_pack(ctx, raw, raw_stride, (int)g.raw_len, n_frames, nseg, ctx->dfl_scratch.as<uint8_t>(), info, start, png,
+                               png_stride, (int)g.idat_data_off + 2));
+    B2_KERNEL(ctx, "png_wrap_kernel");
+    png_wrap_kernel<<<(n_frames + 127) / 128, 128, 0, ctx->stream>>>(g, n_frames, lens, ctx->png_sums.as<uint32_t>(), ihdr_crc(g), png,
+                                                                     png_stride);
+    B2_LAUNCH_CHECK(ctx);
+    B2_KERNEL(ctx, "png_crc_kernel");
+    png_crc_kernel<<<png_grid(ctx, (long long)npiece * n_frames, 128), 128, 0, ctx->stream>>>(png, png_stride, lens, n_frames, npiece, pieces);
+    B2_LAUNCH_CHECK(ctx);
+    B2_KERNEL(ctx, "png_crc_seal_kernel");
+    png_crc_seal_kernel<<<(n_frames + 127) / 128, 128, 0, ctx->stream>>>(pieces, n_frames, npiece, lens, x8nmodp(PNG_SEG), png, png_stride);
+    B2_LAUNCH_CHECK(ctx);
+    *png_lens = lens;
+    return B200TIMG_OK;
+}
+
+// n composed frames (RGBA8, device) -> their framed kitty / iTerm2 text at d_out + d_offsets[f].  Stored blocks:
+// the offsets are already on the device, computed by the caller from b200timg_graphics_size.  B200TIMG_DEFLATE:
+// the offsets are computed here, on the device.
 int launch_graphics(b200timg_ctx *ctx, const uint8_t *d_frames, int w, int h, int n_frames, const b200timg_graphics &gr,
-                    const uint32_t *d_ids, const uint64_t *d_offsets, char *d_out, size_t out_cap) {
+                    const uint32_t *d_ids, uint64_t *d_offsets, char *d_out, size_t out_cap) {
     const PngGeom g = png_geom(w, h, gr.rgb24);
     if (g.png_len > 0x7fffffffll) return ctx->fail(B200TIMG_EINVAL, "graphics: frame too large for one IDAT chunk");
-    B2_TRY(launch_png_sums(ctx, d_frames, g, n_frames, nullptr));
     const GfxSpec s = gfx_spec(gr, g);
-    const uint32_t *ids = gr.protocol == B200TIMG_ITERM2 ? nullptr : d_ids;
+    const uint32_t *ids = s.protocol == B200TIMG_ITERM2 ? nullptr : d_ids;
+    const long long png_stride = (g.png_len + 15) / 16 * 16;
+    uint32_t *png_lens = nullptr;
+    if (gr.protocol & B200TIMG_DEFLATE) B2_TRY(launch_png_deflate(ctx, d_frames, g, n_frames, s, ids, d_offsets, png_stride, &png_lens));
+    else B2_TRY(launch_png_sums(ctx, d_frames, g, n_frames, nullptr));
     const long long tiles = s.tiles * n_frames, cap = (long long)ctx->sm_count * 16;
     B2_KERNEL(ctx, "graphics_emit_kernel");
     graphics_emit_kernel<<<(unsigned)std::min(tiles, cap), GFX_THREADS, 0, ctx->stream>>>(
-        d_frames, g, s, n_frames, ids, ctx->png_sums.as<uint32_t>(), ihdr_crc(g), d_offsets, d_out, (unsigned long long)out_cap);
+        d_frames, g, s, n_frames, ids, ctx->png_sums.as<uint32_t>(), ihdr_crc(g), d_offsets, d_out, (unsigned long long)out_cap,
+        png_lens ? ctx->dfl_png.as<uint8_t>() : nullptr, png_stride, png_lens);
     B2_LAUNCH_CHECK(ctx);
-    if (gr.protocol == B200TIMG_KITTY_TMUX) {
+    if (s.protocol == B200TIMG_KITTY_TMUX) {
         const long long items = (long long)n_frames * s.rows * (s.cols > GRID_CELLS ? (s.cols + GRID_CELLS - 1) / GRID_CELLS : 1);
         B2_KERNEL(ctx, "graphics_grid_kernel");
         graphics_grid_kernel<<<(unsigned)std::min(items, cap), GFX_THREADS, 0, ctx->stream>>>(s, n_frames, ids, d_offsets, d_out,
-                                                                                              (unsigned long long)out_cap);
+                                                                                              (unsigned long long)out_cap, png_lens);
         B2_LAUNCH_CHECK(ctx);
     }
     return B200TIMG_OK;
@@ -610,9 +762,10 @@ size_t b200timg_base64_size(size_t n) { return (n + 2) / 3 * 4; }
 
 size_t b200timg_graphics_size(const b200timg_graphics *g, int w, int h, uint32_t id) {
     if (!g || w <= 0 || h <= 0) return 0;
-    if (g->protocol == B200TIMG_KITTY_TMUX) {
+    const int protocol = g->protocol & ~B200TIMG_DEFLATE;
+    if (protocol == B200TIMG_KITTY_TMUX) {
         if (g->cell_x_px <= 0 || g->cell_y_px <= 0 || g->indent_cells < 0) return 0;
-    } else if (g->protocol != B200TIMG_KITTY && g->protocol != B200TIMG_ITERM2) {
+    } else if (protocol != B200TIMG_KITTY && protocol != B200TIMG_ITERM2) {
         return 0;
     }
     return gfx_frame_size(gfx_spec(*g, png_geom(w, h, g->rgb24)), id);

@@ -7,6 +7,9 @@
   C2-kitty-tmux  the same in kitty's tmux form at 9x18-px cells: passthrough framing and a 300 x 85 placeholder grid
   C2-iterm2      the same through iTerm2
   C4-kitty       3840x2160 RGBA -> 337x190 (C4 geometry), 128 frames, kitty, rgb24, composed onto black
+  *-deflate      the same with B200TIMG_DEFLATE (compressed PNGs), run right after its stored configuration;
+                 encoded bytes against the stored bytes, and the IDAT bytes of 8 sampled frames against zlib level 1
+                 (Python's zlib on the host, same scaled frames)
 
 Per configuration: device-resident Mpx/s of input pixels and encoded GB/s; B_alg = (source bytes + encoded bytes)
 over the chain time, as a share of the H100 SXM's 3350 GB/s (DESIGN.md section 4); the per-kernel ms of one batch
@@ -38,8 +41,46 @@ CONFIGS = {
     "C2-kitty": dict(iw=3840, ih=2160, ow=2700, oh=1519, n=132, proto=timg_b200.KITTY, has_bg=0),
     "C2-kitty-tmux": dict(iw=3840, ih=2160, ow=2700, oh=1519, n=132, proto=timg_b200.KITTY_TMUX, has_bg=0, cell=(9, 18)),
     "C2-iterm2": dict(iw=3840, ih=2160, ow=2700, oh=1519, n=132, proto=timg_b200.ITERM2, has_bg=0),
+    "C2-kitty-deflate": dict(iw=3840, ih=2160, ow=2700, oh=1519, n=132, proto=timg_b200.KITTY, has_bg=0, deflate=True),
+    "C2-iterm2-deflate": dict(iw=3840, ih=2160, ow=2700, oh=1519, n=132, proto=timg_b200.ITERM2, has_bg=0, deflate=True),
     "C4-kitty": dict(iw=3840, ih=2160, ow=337, oh=190, n=128, proto=timg_b200.KITTY, has_bg=1),
+    "C4-kitty-deflate": dict(iw=3840, ih=2160, ow=337, oh=190, n=128, proto=timg_b200.KITTY, has_bg=1, deflate=True),
 }
+ORDER = ["C2-kitty", "C2-kitty-deflate", "C2-kitty-tmux", "C2-iterm2", "C2-iterm2-deflate", "C4-kitty", "C4-kitty-deflate"]
+
+
+def scanlines(fb):
+    """The Sub-filtered rgb24 scanline stream of a frame (the PNG's raw IDAT content, src/timg-png.cc:119-134)."""
+    px = np.ascontiguousarray(fb[..., :3])
+    d = px.copy()
+    d[:, 1:] = px[:, 1:] - px[:, :-1]
+    return np.concatenate([np.ones((px.shape[0], 1), np.uint8), d.reshape(px.shape[0], -1)], axis=1).tobytes()
+
+
+def idat_bytes(text):
+    """IDAT length of the PNG in one framed kitty or iTerm2 frame: its base64 payload, decoded."""
+    import base64
+    import re
+    if text.startswith(b"\033]1337;"):
+        b64 = text[text.index(b":") + 1:text.rindex(b"\a")]
+    else:
+        b64 = b"".join(re.findall(rb"\033_G[^;]*;([A-Za-z0-9+/=]*)\033\\", text))
+    return int.from_bytes(base64.b64decode(b64)[33:37], "big")
+
+
+def zlib1_ratio(torch, L, ctx, d_src, b, cfg, out, offs, n):
+    """IDAT bytes of 8 sampled frames over zlib level 1's stream of the same scanlines."""
+    import zlib
+    ow, oh = cfg["ow"], cfg["oh"]
+    d_fb = torch.empty((n, oh, ow, 4), dtype=torch.uint8, device="cuda")
+    ctx._chk(L.b200timg_scale_dev(ctx.h, d_src.data_ptr(), cfg["iw"], cfg["ih"], 0, d_fb.data_ptr(), ow, oh, n))
+    ctx._chk(L.b200timg_compose_dev(ctx.h, d_fb.data_ptr(), ow, oh, n, cfg["has_bg"], b.bg, 0, 0, 0, 0))
+    torch.cuda.synchronize()
+    ours = ref = 0
+    for f in range(0, n, max(1, n // 8))[:8]:
+        ours += idat_bytes(out[int(offs[f]):int(offs[f + 1])].tobytes())
+        ref += len(zlib.compress(scanlines(d_fb[f].cpu().numpy()), 1))
+    return round(ours / ref, 4)
 
 
 def gpu_info():
@@ -85,7 +126,8 @@ def run(name, cfg, steps, warmup, torch):
                         bg=timg_b200.rgba_u32(0, 0, 0), pattern=0, pattern_w=0, pattern_h=0, flags=0, x_indent_cells=0,
                         animation=0)
     ids = np.arange(1, n + 1, dtype=np.uint32) + np.uint32(1_700_000_000)
-    g, keep = timg_b200.graphics(proto, True, ids, cfg.get("cell"))
+    deflate = cfg.get("deflate", False)
+    g, keep = timg_b200.graphics(proto | (timg_b200.DEFLATE if deflate else 0), True, ids, cfg.get("cell"))
     d_src = frames_on_device(torch, iw, ih, n)
     total = sum(L.b200timg_graphics_size(C.byref(g), ow, oh, int(i)) for i in ids)
     d_out = torch.empty(total, dtype=torch.uint8, device="cuda")
@@ -102,7 +144,8 @@ def run(name, cfg, steps, warmup, torch):
         step()
     torch.cuda.synchronize()
     ms = (time.perf_counter() - t0) * 1e3 / steps
-    assert int(d_offs[-1]) == total
+    encoded = int(d_offs[-1])
+    assert encoded == total or deflate and encoded <= total
     src_bytes = n * iw * ih * 4
     ctx.profile(True)
     step()
@@ -119,14 +162,17 @@ def run(name, cfg, steps, warmup, torch):
         ctx._chk(L.b200timg_graphics_batch(ctx.h, C.byref(b), C.byref(g), h_src.ctypes.data, out.ctypes.data, total,
                                            offs.ctypes.data))
     host_s = (time.perf_counter() - t0) / steps
-    same = out.tobytes() == d_out.cpu().numpy().tobytes()
+    same = out[:encoded].tobytes() == d_out[:encoded].cpu().numpy().tobytes() and bool((offs == d_offs.cpu().numpy().astype(np.uint64)).all())
     result = dict(config=name, frames=n, src=f"{iw}x{ih}", out=f"{ow}x{oh}", protocol=PROTOCOL_NAMES[proto],
-                  rgb24=True, has_bg=bool(cfg["has_bg"]), encoded_bytes=total, steps=steps,
-                  dev_ms=round(ms, 3), dev_mpx_s=round(n * iw * ih / ms / 1e3, 1), dev_encoded_gbs=round(total / ms / 1e6, 2),
-                  b_alg_gbs=round((src_bytes + total) / ms / 1e6, 1), b_alg_share=round((src_bytes + total) / ms / 1e6 / HBM_GBS, 4),
+                  rgb24=True, has_bg=bool(cfg["has_bg"]), deflate=deflate, encoded_bytes=encoded, stored_bytes=total,
+                  encoded_over_stored=round(encoded / total, 4), steps=steps,
+                  dev_ms=round(ms, 3), dev_mpx_s=round(n * iw * ih / ms / 1e3, 1), dev_encoded_gbs=round(encoded / ms / 1e6, 2),
+                  b_alg_gbs=round((src_bytes + encoded) / ms / 1e6, 1), b_alg_share=round((src_bytes + encoded) / ms / 1e6 / HBM_GBS, 4),
                   kernels_ms=kernels, host_e2e_ms=round(host_s * 1e3, 2), host_e2e_mpx_s=round(n * iw * ih / host_s / 1e6, 1),
                   host_equals_dev=same, png_batch_route=None)
-    if proto == timg_b200.KITTY_TMUX:
+    if deflate:
+        result["idat_over_zlib1"] = zlib1_ratio(torch, L, ctx, d_src, b, cfg, out, offs, n)
+    if proto == timg_b200.KITTY_TMUX or deflate:
         ctx.close()
         return result
 
@@ -175,10 +221,10 @@ def main():
     a = ap.parse_args()
     import torch
     info = gpu_info()
-    for name, cfg in CONFIGS.items():
+    for name in ORDER:
         if a.only and name != a.only:
             continue
-        r = run(name, cfg, a.steps, a.warmup, torch)
+        r = run(name, CONFIGS[name], a.steps, a.warmup, torch)
         r["gpu"] = info
         print(json.dumps(r), flush=True)
         torch.cuda.empty_cache()
