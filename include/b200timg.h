@@ -232,6 +232,53 @@ int b200timg_blocks_batch(b200timg_ctx *ctx, const b200timg_batch *b, const uint
 int b200timg_sixel_batch(b200timg_ctx *ctx, const b200timg_batch *b, const uint8_t *src,
                          char *out, size_t out_cap, uint64_t *offsets);
 
+/* ======================= mixed batches: one grid page of differently sized images ====================
+ * The batches above share one geometry.  A page of `timg --grid=CxR a.jpg b.png ...` does not: every image has its own
+ * source size, its own b200timg_calc_fit result for the grid's per-image box (src/timg.cc:938-939) and its own x
+ * position (src/renderer.cc:103-148: column offset plus centering).  A mixed batch describes such a page: frame f has
+ * its own source and output geometry and indent, the page shares the colour format, the block flags and the
+ * compose options (one DisplayOptions).  Frame f's bytes are exactly those of the single-frame path on that image
+ * (ImageScaler::Scale -> AlphaComposeBackground -> UnicodeBlockCanvas::Send of a full frame, as the uniform batch
+ * composes them), whatever the frame's place in the batch, the batch size or the variant called.  A call runs a fixed
+ * number of kernels and uploads its tables and descriptors in one copy, however many geometries the page has; frames
+ * of equal geometry share one resampling plan.  The scaler's float intermediate is bounded: a page whose
+ * intermediate exceeds 2 GiB runs as several frame groups (the count depends on bytes, never on geometries).
+ * Source frames: RGBA or RGB32, tightly packed, frame f at src + frames[f].src_offset.
+ * Rejected with B200TIMG_EINVAL: n_frames <= 0 or > 65535, frames == NULL, a non-positive size, a negative indent, a
+ * src_offset that is not a multiple of 4, an odd out_w in quarter mode (the message names the frame), a YUV or
+ * unknown src_fmt, B200TIMG_BILINEAR_SCALE, more than 2^31 - 1 row pairs or scaler work items in one call.
+ * B200TIMG_FAST_SCALE is accepted and ignored: mixed batches always scale bit-exactly.
+ * Out of scope: delta frames (a grid page has none, so there is no animation field), YUV sources, the bilinear
+ * scaler, and the sixel / kitty / iTerm2 encoders (they build on b200timg_scale_mixed_dev's output). */
+typedef struct {
+    uint64_t src_offset;        /* bytes from the batch's source pointer to this frame's first pixel; multiple of 4 */
+    int src_w, src_h;           /* source geometry of this image */
+    int out_w, out_h;           /* its b200timg_calc_fit result */
+    int x_indent_cells;         /* UnicodeBlockCanvas::Send's x after "x /= 2" for this image (column offset + centering) */
+} b200timg_frame;
+
+typedef struct {
+    int n_frames;
+    int src_fmt;                /* B200TIMG_FMT_RGBA or B200TIMG_FMT_RGB32 */
+    int flags;                  /* B200TIMG_QUARTER | _UPPER | _COLOR8 (| _FAST_SCALE: accepted, computed exactly) */
+    int has_bg;                 /* compose, shared by the page: as b200timg_batch */
+    uint32_t bg, pattern;
+    int pattern_w, pattern_h;
+    const b200timg_frame *frames;   /* HOST pointer, n_frames entries */
+} b200timg_mixed_batch;
+
+/* Scale + fused compose of every frame (DEVICE pointers, asynchronous): frame f's out_w*out_h*4 bytes land at d_out
+ * plus the sum of the earlier frames' out_w*out_h*4; d_src and d_out 4-byte aligned. */
+int b200timg_scale_mixed_dev(b200timg_ctx *ctx, const b200timg_mixed_batch *b, const uint8_t *d_src, uint8_t *d_out);
+/* scale -> compose -> half/quarter blocks; frames back to back, offsets[n_frames + 1] as in the uniform batches.
+ * The _dev variant follows the OUTPUT CAPACITY CONTRACT above; the sum of b200timg_blocks_bound(out_w, out_h) over the
+ * frames cannot overflow.  The host variant returns B200TIMG_ENOSPC with offsets[] complete (offsets[n_frames] = the
+ * bytes needed) and writes nothing at or beyond out_cap. */
+int b200timg_blocks_mixed_dev(b200timg_ctx *ctx, const b200timg_mixed_batch *b, const uint8_t *d_src,
+                              char *d_out, size_t out_cap, uint64_t *d_offsets);
+int b200timg_blocks_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *b, const uint8_t *src,
+                          char *out, size_t out_cap, uint64_t *offsets);
+
 /* Device-resident single stages, for tests and for callers that keep frames on the GPU
  * (e.g. an NVDEC front end).  All pointers are DEVICE pointers. */
 int b200timg_scale_dev(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int fmt,

@@ -56,6 +56,16 @@ class Graphics(C.Structure):
                 ("cell_x_px", C.c_int), ("cell_y_px", C.c_int), ("indent_cells", C.c_int)]
 
 
+class Frame(C.Structure):
+    _fields_ = [("src_offset", C.c_uint64), ("src_w", C.c_int), ("src_h", C.c_int), ("out_w", C.c_int), ("out_h", C.c_int),
+                ("x_indent_cells", C.c_int)]
+
+
+class MixedBatch(C.Structure):
+    _fields_ = [("n_frames", C.c_int), ("src_fmt", C.c_int), ("flags", C.c_int), ("has_bg", C.c_int), ("bg", C.c_uint32),
+                ("pattern", C.c_uint32), ("pattern_w", C.c_int), ("pattern_h", C.c_int), ("frames", C.POINTER(Frame))]
+
+
 # name -> (restype, argtypes); this table IS the list of exported symbols tests check.
 ABI = {
     "b200timg_version": (C.c_int, []),
@@ -88,6 +98,9 @@ ABI = {
                                         C.c_void_p]),
     "b200timg_sixel_batch": (C.c_int, [C.c_void_p, C.POINTER(Batch), C.c_void_p, C.c_void_p, C.c_size_t,
                                        C.c_void_p]),
+    "b200timg_scale_mixed_dev": (C.c_int, [C.c_void_p, C.POINTER(MixedBatch), C.c_void_p, C.c_void_p]),
+    "b200timg_blocks_mixed_dev": (C.c_int, [C.c_void_p, C.POINTER(MixedBatch), C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200timg_blocks_mixed": (C.c_int, [C.c_void_p, C.POINTER(MixedBatch), C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200timg_scale_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                      C.c_int, C.c_int]),
     "b200timg_compose_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint32,
@@ -214,6 +227,43 @@ def _source_frames(frames):
     if frames.dtype == np.uint16:
         return frames.reshape(frames.shape[0], -1).view(np.uint8)
     return np.ascontiguousarray(frames, dtype=np.uint8)
+
+
+def pack_mixed(images):
+    """Source frames of differing shapes ([h, w, 4] uint8 each) back to back in one uint8 array, and each frame's byte
+    offset (whole RGBA frames keep every offset a multiple of 4)."""
+    images = [np.ascontiguousarray(im, dtype=np.uint8) for im in images]
+    offsets = np.cumsum([0] + [im.nbytes for im in images])
+    flat = np.empty(max(1, int(offsets[-1])), np.uint8)
+    for im, o in zip(images, offsets):
+        flat[int(o):int(o) + im.nbytes] = im.reshape(-1)
+    return flat, [int(o) for o in offsets[:-1]]
+
+
+def mixed_batch(shapes, outs, src_offsets, indents=None, flags=0, src_fmt=FMT_RGBA, has_bg=True, bg=0xFF000000, pattern=0,
+                pattern_w=0, pattern_h=0):
+    """(b200timg_mixed_batch, its frame array): keep both alive for the call.  shapes: each source's (h, w[, 4]); outs:
+    each frame's (out_w, out_h); indents: each frame's x_indent_cells (default 0)."""
+    n = len(outs)
+    frames = (Frame * max(1, n))()
+    for f in range(n):
+        h, w = shapes[f][:2]
+        frames[f] = Frame(src_offsets[f], w, h, outs[f][0], outs[f][1], indents[f] if indents is not None else 0)
+    return MixedBatch(n, src_fmt, flags, int(has_bg), bg, pattern, pattern_w, pattern_h, frames), frames
+
+
+def _device_tensor(torch, a):
+    """Device copy of a numpy array for the _dev entry points.  torch without CUDA only reaches here under the CPU kernel
+    simulator (tools/cusim), whose device memory is host memory: a Context cannot exist otherwise."""
+    t = torch.from_numpy(np.ascontiguousarray(a))
+    return t.cuda() if torch.cuda.is_available() else t.clone()
+
+
+def device_sync(torch):
+    """Wait for every stream of the device, the context's own included (torch's copies run on torch's stream, which
+    does not wait for the context's).  Nothing to wait for under the CPU kernel simulator."""
+    if torch.cuda.is_available():
+        torch.cuda.synchronize()
 
 
 class Context:
@@ -397,6 +447,55 @@ class Context:
                                                 offs.ctypes.data))
         res = [out[int(offs[i]):int(offs[i + 1])].tobytes() for i in range(n)]
         return (res, offs) if with_offsets else res
+
+    # ---- mixed batches: images of differing geometry (numpy [h, w, 4] each)
+    def scale_mixed(self, images, outs, src_fmt=FMT_RGBA, has_bg=True, bg=0xFF000000, pattern=0, pattern_w=0, pattern_h=0):
+        """b200timg_scale_mixed_dev on the packed images: the scaled, composed frames as a list of [oh, ow, 4] arrays."""
+        import torch
+        flat, offs = pack_mixed(images)
+        b, keep = mixed_batch([im.shape for im in images], outs, offs, None, 0, src_fmt, has_bg, bg, pattern, pattern_w,
+                              pattern_h)
+        d_src = _device_tensor(torch, flat)
+        sizes = [ow * oh * 4 for ow, oh in outs]
+        d_out = torch.empty(max(1, sum(sizes)), dtype=torch.uint8, device=d_src.device)
+        self._chk(lib().b200timg_scale_mixed_dev(self.h, C.byref(b), d_src.data_ptr(), d_out.data_ptr()))
+        device_sync(torch)
+        host = d_out.cpu().numpy()
+        res, o = [], 0
+        for (ow, oh), n in zip(outs, sizes):
+            res.append(host[o:o + n].reshape(oh, ow, 4).copy())
+            o += n
+        return res
+
+    def blocks_mixed(self, images, outs, indents=None, flags=0, src_fmt=FMT_RGBA, has_bg=True, bg=0xFF000000, pattern=0,
+                     pattern_w=0, pattern_h=0):
+        """b200timg_blocks_mixed (host buffers): each frame's block bytes, as a list of bytes."""
+        flat, offs = pack_mixed(images)
+        b, keep = mixed_batch([im.shape for im in images], outs, offs, indents, flags, src_fmt, has_bg, bg, pattern,
+                              pattern_w, pattern_h)
+        n = len(outs)
+        cap = sum(lib().b200timg_blocks_bound(ow, oh) for ow, oh in outs) + 64
+        out = np.empty(cap, np.uint8)
+        o = np.zeros(n + 1, np.uint64)
+        self._chk(lib().b200timg_blocks_mixed(self.h, C.byref(b), flat.ctypes.data, out.ctypes.data, cap, o.ctypes.data))
+        return [out[int(o[i]):int(o[i + 1])].tobytes() for i in range(n)]
+
+    def blocks_mixed_dev(self, d_src, b, d_out=None, out_cap=None, d_offsets=None):
+        """b200timg_blocks_mixed_dev on a packed source tensor (see pack_mixed / mixed_batch): returns (d_out, d_offsets)
+        after the (asynchronous) call -- device_sync() before reading them; d_out defaults to the sum of the frames' block
+        bounds."""
+        import torch
+        n = b.n_frames
+        if d_out is None:
+            cap = sum(lib().b200timg_blocks_bound(b.frames[f].out_w, b.frames[f].out_h) for f in range(n))
+            d_out = torch.empty(cap, dtype=torch.uint8, device=d_src.device)
+        if out_cap is None:
+            out_cap = d_out.numel()
+        if d_offsets is None:
+            d_offsets = torch.empty(n + 1, dtype=torch.int64, device=d_src.device)
+        self._chk(lib().b200timg_blocks_mixed_dev(self.h, C.byref(b), d_src.data_ptr(), d_out.data_ptr(), out_cap,
+                                                  d_offsets.data_ptr()))
+        return d_out, d_offsets
 
     def graphics_batch_dev(self, d_src, b, protocol, rgb24=False, ids=None, d_out=None, out_cap=None, d_offsets=None,
                            cell=None, indent=0):

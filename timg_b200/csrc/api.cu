@@ -74,6 +74,8 @@ void b200timg_ctx_destroy(b200timg_ctx *ctx) {
     ctx->in_stage.release(); ctx->fb_scaled.release(); ctx->prev_stage.release();
     ctx->out_stage.release(); ctx->offsets.release(); ctx->cells.release(); ctx->rows.release();
     ctx->tables.release(); ctx->sixel_work.release(); ctx->misc.release(); ctx->scale_list.release(); ctx->scale_tmp.release(); ctx->tri_tables.release();
+    ctx->mixed_arena.release(); ctx->mixed_stage.release();
+    if (ctx->ev_mixed) cudaEventDestroy(ctx->ev_mixed);
     ctx->pinned.release(); ctx->pinned_io.release();
     ctx->png_sums.release(); ctx->gfx_ids.release();
     ctx->dfl_raw.release(); ctx->dfl_scratch.release(); ctx->dfl_meta.release(); ctx->dfl_tokens.release(); ctx->dfl_png.release();
@@ -707,6 +709,104 @@ static int batch_host_impl(b200timg_ctx *ctx, const b200timg_batch *b, const uin
         B2_TRY(sync(ctx));
         return ctx->fail(B200TIMG_ENOSPC, "batch: need %zu bytes (have %zu)", base_bytes, out_cap);
     }
+    return sync(ctx);
+}
+
+// ---- mixed batches ------------------------------------------------------------------------------------------------
+static int validate_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *b, bool blocks) {
+    if (!b || b->n_frames <= 0 || !b->frames)
+        return ctx->fail(B200TIMG_EINVAL, "mixed batch: needs n_frames > 0 and a frames array (n_frames %d, frames %s)",
+                         b ? b->n_frames : 0, b && b->frames ? "set" : "NULL");
+    if (b->n_frames > 65535) return ctx->fail(B200TIMG_EINVAL, "mixed batch: %d frames, at most 65535 per call", b->n_frames);
+    if (b->src_fmt != B200TIMG_FMT_RGBA && b->src_fmt != B200TIMG_FMT_RGB32)
+        return ctx->fail(B200TIMG_EINVAL, "mixed batch: source format %d is not RGBA or RGB32 (YUV sources are not supported)", b->src_fmt);
+    if (b->flags & B200TIMG_BILINEAR_SCALE)
+        return ctx->fail(B200TIMG_EINVAL, "mixed batch: B200TIMG_BILINEAR_SCALE is not supported (the STB scaler only)");
+    for (int f = 0; f < b->n_frames; ++f) {
+        const b200timg_frame &F = b->frames[f];
+        if (F.src_w <= 0 || F.src_h <= 0 || F.out_w <= 0 || F.out_h <= 0)
+            return ctx->fail(B200TIMG_EINVAL, "mixed batch: frame %d: non-positive size %dx%d -> %dx%d", f, F.src_w, F.src_h, F.out_w, F.out_h);
+        if (F.src_offset & 3)
+            return ctx->fail(B200TIMG_EINVAL, "mixed batch: frame %d: src_offset %llu is not a multiple of 4", f,
+                             (unsigned long long)F.src_offset);
+        if (F.x_indent_cells < 0) return ctx->fail(B200TIMG_EINVAL, "mixed batch: frame %d: negative indent %d", f, F.x_indent_cells);
+        if (blocks && (b->flags & B200TIMG_QUARTER) && (F.out_w & 1))
+            return ctx->fail(B200TIMG_EINVAL, "mixed batch: frame %d: quarter blocks need an even width (got %d); the "
+                             "reference reads past the row end there", f, F.out_w);
+    }
+    return B200TIMG_OK;
+}
+
+// The plan's one upload.  The pinned staging is rewritten only after the previous mixed call's copy has run.
+static int mixed_upload(b200timg_ctx *ctx, const MixedPlan &mp) {
+    if (ctx->ev_mixed) B2_CUDA(ctx, cudaEventSynchronize(ctx->ev_mixed));
+    else B2_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_mixed, cudaEventDisableTiming));
+    B2_CUDA(ctx, ctx->mixed_stage.reserve(mp.arena.size()));
+    B2_CUDA(ctx, ctx->mixed_arena.reserve(mp.arena.size()));
+    memcpy(ctx->mixed_stage.p, mp.arena.data(), mp.arena.size());
+    B2_CUDA(ctx, cudaMemcpyAsync(ctx->mixed_arena.p, ctx->mixed_stage.p, mp.arena.size(), cudaMemcpyHostToDevice, ctx->stream));
+    B2_CUDA(ctx, cudaEventRecord(ctx->ev_mixed, ctx->stream));
+    return B200TIMG_OK;
+}
+
+int b200timg_scale_mixed_dev(b200timg_ctx *ctx, const b200timg_mixed_batch *b, const uint8_t *d_src, uint8_t *d_out) {
+    B2_TRY(check_ctx(ctx));
+    B2_TRY(validate_mixed(ctx, b, false));
+    if (!d_src || !d_out) return ctx->fail(B200TIMG_EINVAL, "mixed batch: null pointer");
+    if ((reinterpret_cast<uintptr_t>(d_src) | reinterpret_cast<uintptr_t>(d_out)) & 3)
+        return ctx->fail(B200TIMG_EINVAL, "mixed batch: pixel buffers must be 4-byte aligned");
+    MixedPlan mp;
+    B2_TRY(plan_scale_mixed(ctx, b, mp));
+    B2_TRY(mixed_upload(ctx, mp));
+    const ComposeSpec cs = make_compose_spec(b->has_bg, b->bg, b->pattern, b->pattern_w, b->pattern_h);
+    return launch_scale_mixed(ctx, mp, ctx->mixed_arena.as<char>(), d_src, d_out, b->n_frames, b->src_fmt == B200TIMG_FMT_RGB32, cs);
+}
+
+int b200timg_blocks_mixed_dev(b200timg_ctx *ctx, const b200timg_mixed_batch *b, const uint8_t *d_src,
+                              char *d_out, size_t out_cap, uint64_t *d_offsets) {
+    B2_TRY(check_ctx(ctx));
+    B2_TRY(validate_mixed(ctx, b, true));
+    if (!d_src || !d_out || !d_offsets) return ctx->fail(B200TIMG_EINVAL, "mixed batch: null pointer");
+    if (reinterpret_cast<uintptr_t>(d_src) & 3) return ctx->fail(B200TIMG_EINVAL, "mixed batch: pixel buffers must be 4-byte aligned");
+    MixedPlan mp;
+    B2_TRY(plan_scale_mixed(ctx, b, mp));
+    B2_TRY(plan_blocks_mixed(ctx, b, mp));
+    ctx->resident_fb = nullptr;
+    B2_CUDA(ctx, ctx->fb_scaled.reserve((size_t)mp.out_px * 4));
+    B2_TRY(mixed_upload(ctx, mp));
+    const ComposeSpec cs = make_compose_spec(b->has_bg, b->bg, b->pattern, b->pattern_w, b->pattern_h);
+    uint8_t *d_fb = ctx->fb_scaled.as<uint8_t>();
+    B2_TRY(launch_scale_mixed(ctx, mp, ctx->mixed_arena.as<char>(), d_src, d_fb, b->n_frames, b->src_fmt == B200TIMG_FMT_RGB32, cs));
+    return launch_blocks_mixed(ctx, mp, ctx->mixed_arena.as<char>(), d_fb, b->n_frames, b->flags, d_out, out_cap, d_offsets);
+}
+
+// Host buffers: upload the sources, run the device variant into staging bounded by the sum of the frames' block bounds,
+// read the offsets, then download exactly the encoded bytes (or nothing, with ENOSPC).
+int b200timg_blocks_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *b, const uint8_t *src,
+                          char *out, size_t out_cap, uint64_t *offsets) {
+    B2_TRY(check_ctx(ctx));
+    B2_TRY(validate_mixed(ctx, b, true));
+    if (!src || !out || !offsets) return ctx->fail(B200TIMG_EINVAL, "mixed batch: null pointer");
+    const int n = b->n_frames;
+    size_t src_bytes = 0, bound = 64;
+    for (int f = 0; f < n; ++f) {
+        const b200timg_frame &F = b->frames[f];
+        src_bytes = std::max(src_bytes, (size_t)F.src_offset + (size_t)F.src_w * F.src_h * 4);
+        bound += b200timg_blocks_bound(F.out_w, F.out_h);
+    }
+    B2_CUDA(ctx, ctx->in_stage.reserve(src_bytes));
+    B2_CUDA(ctx, ctx->out_stage.reserve(bound));
+    B2_CUDA(ctx, ctx->offsets.reserve((size_t)(n + 1) * sizeof(uint64_t)));
+    B2_CUDA(ctx, ctx->pinned.reserve((size_t)(n + 1) * sizeof(uint64_t)));
+    B2_TRY(upload(ctx, ctx->in_stage.p, src, src_bytes));
+    B2_TRY(b200timg_blocks_mixed_dev(ctx, b, ctx->in_stage.as<uint8_t>(), ctx->out_stage.as<char>(), bound, ctx->offsets.as<uint64_t>()));
+    B2_TRY(download(ctx, ctx->pinned.p, ctx->offsets.p, (size_t)(n + 1) * sizeof(uint64_t)));
+    B2_TRY(sync(ctx));
+    memcpy(offsets, ctx->pinned.p, (size_t)(n + 1) * sizeof(uint64_t));
+    const size_t total = (size_t)offsets[n];
+    if (total > bound) return ctx->fail(B200TIMG_ECUDA, "mixed batch: encoded size %zu exceeds the bound %zu", total, bound);
+    if (total > out_cap) return ctx->fail(B200TIMG_ENOSPC, "mixed batch: need %zu bytes (have %zu)", total, out_cap);
+    if (total) B2_TRY(download(ctx, out, ctx->out_stage.p, total));
     return sync(ctx);
 }
 

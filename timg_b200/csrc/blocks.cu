@@ -181,42 +181,117 @@ struct BlocksParams {
 
 constexpr int BT = 256;
 
+// The frame that owns flat item `item`: the last f with start[f] <= item (frames without items share their start).
+__device__ __forceinline__ int mixed_owner(const unsigned *__restrict__ start, int n, unsigned item) {
+    int lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (start[mid] <= item) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
+// Where a CTA's row pair and its frame live.  The pass bodies below read every per-frame quantity through one of
+// these accessors:
+//   UniformGeom  a b200timg_batch: every frame has P's geometry, frame f at fb + f * P.frame_px, records frame-major
+//   MixedGeom    a mixed batch: each frame has its own geometry and record offsets (MixedBlocksFrame), no delta frames
+struct UniformGeom {
+    typedef BlocksParams Params;
+    const BlocksParams &P;
+    int f, r;                             // frame, row pair
+    __device__ __forceinline__ UniformGeom(const BlocksParams &p, int f_, int r_) : P(p), f(f_), r(r_) {}
+    __device__ __forceinline__ explicit UniformGeom(const BlocksParams &p) : P(p), f(blockIdx.y), r(blockIdx.x) {}
+    __device__ __forceinline__ int quarter() const { return P.quarter; }
+    __device__ __forceinline__ int upper() const { return P.upper; }
+    __device__ __forceinline__ int color8() const { return P.color8; }
+    __device__ __forceinline__ int w() const { return P.w; }
+    __device__ __forceinline__ int h() const { return P.h; }
+    __device__ __forceinline__ int cols() const { return P.cols; }
+    __device__ __forceinline__ int rows() const { return P.rows; }
+    __device__ __forceinline__ int row_offset() const { return P.row_offset; }
+    __device__ __forceinline__ int indent() const { return P.indent; }
+    __device__ __forceinline__ int prev_mode() const { return P.prev_mode; }
+    __device__ __forceinline__ long long frame_px0() const { return (long long)f * P.frame_px; }        // first pixel
+    __device__ __forceinline__ long long prev_px0() const { return (long long)(f - 1) * P.frame_px; }
+    __device__ __forceinline__ long long first_row_rec() const { return (long long)f * P.rows; }
+    __device__ __forceinline__ long long first_cell_rec() const { return ((long long)f * P.rows + r) * P.cols; }
+};
+
+struct MixedBlocksParams {
+    const MixedBlocksFrame *desc;
+    const unsigned *row_start;            // [n_frames + 1] first (frame, row pair) item of each frame
+    int n_frames, flags;
+};
+struct MixedGeom {
+    typedef MixedBlocksParams Params;
+    MixedBlocksFrame D;
+    unsigned row0;                        // the frame's first row record (its first flat item)
+    int f, r, flags;
+    __device__ __forceinline__ MixedGeom(const MixedBlocksFrame *frames, const unsigned *row_start, int f_, int r_)
+        : D(frames[f_]), row0(row_start[f_]), f(f_), r(r_), flags(0) {}
+    // one CTA per flat item blockIdx.x
+    __device__ __forceinline__ explicit MixedGeom(const MixedBlocksParams &Q) : flags(Q.flags) {
+        f = mixed_owner(Q.row_start, Q.n_frames, blockIdx.x);
+        row0 = Q.row_start[f];
+        r = (int)(blockIdx.x - row0);
+        D = Q.desc[f];
+    }
+    __device__ __forceinline__ int quarter() const { return flags & B200TIMG_QUARTER; }
+    __device__ __forceinline__ int upper() const { return flags & B200TIMG_UPPER; }
+    __device__ __forceinline__ int color8() const { return flags & B200TIMG_COLOR8; }
+    __device__ __forceinline__ int w() const { return D.w; }
+    __device__ __forceinline__ int h() const { return D.h; }
+    __device__ __forceinline__ int cols() const { return D.cols; }
+    __device__ __forceinline__ int rows() const { return D.rows; }
+    __device__ __forceinline__ int row_offset() const { return D.row_offset; }
+    __device__ __forceinline__ int indent() const { return D.indent; }
+    __device__ __forceinline__ int prev_mode() const { return 0; }
+    __device__ __forceinline__ long long frame_px0() const { return (long long)D.fb_px; }
+    __device__ __forceinline__ long long prev_px0() const { return 0; }                                  // never read: no delta
+    __device__ __forceinline__ long long first_row_rec() const { return row0; }
+    __device__ __forceinline__ long long first_cell_rec() const { return (long long)D.cell0 + (long long)r * D.cols; }
+};
+
+// pass A.  A kernel template rather than a body shared by two kernels (as rowscan and emit are): this way the uniform
+// instantiation is optimised as one function, exactly as before the mixed form existed, and compiles to the same SASS.
+template <class G>
 __global__ void __launch_bounds__(BT)
 blocks_pick_kernel(const uint32_t *__restrict__ fb, const uint32_t *__restrict__ prev_single,
-                   BlocksParams P, CellRec *__restrict__ cells, RowRec *__restrict__ rows) {
+                   typename G::Params P, CellRec *__restrict__ cells, RowRec *__restrict__ rows) {
     __shared__ int s_i[16];
     __shared__ uint32_t s_u[8];
     __shared__ uint32_t s_fg[BT], s_bg[BT];
     __shared__ int c_last_emit, c_last_fgidx;
     __shared__ uint32_t c_last_bg, c_last_fg, c_run;
 
-    const int r = blockIdx.x, f = blockIdx.y, tid = threadIdx.x;
-    const uint32_t *frame = fb + (long long)f * P.frame_px;
+    const G g(P);
+    const int r = g.r, f = g.f, tid = threadIdx.x;
+    const uint32_t *frame = fb + g.frame_px0();
     const uint32_t *prev = nullptr;
-    if (P.prev_mode == 1) prev = prev_single;
-    else if (P.prev_mode >= 2 && f > 0) prev = fb + (long long)(f - 1) * P.frame_px;
+    if (g.prev_mode() == 1) prev = prev_single;
+    else if (g.prev_mode() >= 2 && f > 0) prev = fb + g.prev_px0();
 
-    const int top_row = 2 * r + P.row_offset, bot_row = top_row + 1;
-    const bool top_ok = top_row >= 0, bot_ok = bot_row < P.h;
-    const uint32_t *trow = frame + (long long)top_row * P.w, *brow = frame + (long long)bot_row * P.w;
-    const uint32_t *ptrow = prev ? prev + (long long)top_row * P.w : nullptr;
-    const uint32_t *pbrow = prev ? prev + (long long)bot_row * P.w : nullptr;
+    const int top_row = 2 * r + g.row_offset(), bot_row = top_row + 1;
+    const bool top_ok = top_row >= 0, bot_ok = bot_row < g.h();
+    const uint32_t *trow = frame + (long long)top_row * g.w(), *brow = frame + (long long)bot_row * g.w();
+    const uint32_t *ptrow = prev ? prev + (long long)top_row * g.w() : nullptr;
+    const uint32_t *pbrow = prev ? prev + (long long)bot_row * g.w() : nullptr;
 
     if (tid == 0) { c_last_emit = -1; c_last_fgidx = -1; c_last_bg = 0; c_last_fg = 0; c_run = 0; }
     __syncthreads();
 
-    CellRec *crow = cells + ((long long)f * P.rows + r) * P.cols;
-    const bool upper = P.upper != 0, color8 = P.color8 != 0;
+    CellRec *crow = cells + g.first_cell_rec();
+    const bool upper = g.upper() != 0, color8 = g.color8() != 0;
 
-    for (int c0 = 0; c0 < P.cols; c0 += BT) {
+    for (int c0 = 0; c0 < g.cols(); c0 += BT) {
         const int c = c0 + tid;
-        const bool valid = c < P.cols;
+        const bool valid = c < g.cols();
         bool skipped = true;
         Pick pk; pk.fg = 0; pk.bg = 0; pk.block = kBackground;
         if (valid) {
             uint32_t t0 = 0, t1 = 0, b0 = 0, b1 = 0;
             bool same = prev != nullptr;
-            if (P.quarter) {
+            if (g.quarter()) {
                 if (top_ok) { const uint2 v = *reinterpret_cast<const uint2 *>(trow + 2 * c); t0 = v.x; t1 = v.y; }
                 if (bot_ok) { const uint2 v = *reinterpret_cast<const uint2 *>(brow + 2 * c); b0 = v.x; b1 = v.y; }
                 if (prev) {
@@ -266,7 +341,7 @@ blocks_pick_kernel(const uint32_t *__restrict__ fb, const uint32_t *__restrict__
             const bool emit_fg = (pk.block != kBackground) && (!have_fg || pk.fg != prev_fg);   // :270-279
             const bool emit_bg = !have_emit || pk.bg != prev_bg;                                // :282-297
             const bool bgt = transparent(pk.bg);
-            const uint32_t xskip = have_emit ? (uint32_t)(c - prev_idx - 1) : (uint32_t)(c + P.indent);
+            const uint32_t xskip = have_emit ? (uint32_t)(c - prev_idx - 1) : (uint32_t)(c + g.indent());
             len = (xskip > 0 ? 3 + ndig(xskip) : 0)
                 + ((emit_fg || emit_bg) ? 2 : 0)
                 + (emit_fg ? 5 + color_len(pk.fg, color8) : 0)
@@ -293,23 +368,24 @@ blocks_pick_kernel(const uint32_t *__restrict__ fb, const uint32_t *__restrict__
         RowRec rr; rr.nonempty = c_last_emit >= 0 ? 1u : 0u;
         rr.len = rr.nonempty ? c_run + 5 : 0;     // + "\033[0m\n" (:313-318)
         rr.off = 0; rr.yskip = 0;
-        rows[(long long)f * P.rows + r] = rr;
+        rows[g.first_row_rec() + r] = rr;
     }
 }
 
-__global__ void __launch_bounds__(BT)
-blocks_rowscan_kernel(BlocksParams P, RowRec *__restrict__ rows, FrameRec *__restrict__ frames) {
+
+template <class G>
+__device__ __forceinline__ void blocks_rowscan(const G &g, RowRec *__restrict__ rows, FrameRec *__restrict__ frames) {
     __shared__ int s_i[16];
     __shared__ uint32_t s_u[8];
     __shared__ int s_l[8];
     __shared__ int c_last; __shared__ uint32_t c_run;
-    const int f = blockIdx.x, tid = threadIdx.x;
-    RowRec *rr = rows + (long long)f * P.rows;
+    const int f = g.f, tid = threadIdx.x;
+    RowRec *rr = rows + g.first_row_rec();
     if (tid == 0) { c_last = -1; c_run = 0; }
     __syncthreads();
-    for (int r0 = 0; r0 < P.rows; r0 += BT) {
+    for (int r0 = 0; r0 < g.rows(); r0 += BT) {
         const int r = r0 + tid;
-        const bool valid = r < P.rows;
+        const bool valid = r < g.rows();
         RowRec me; me.len = 0; me.nonempty = 0; me.off = 0; me.yskip = 0;
         if (valid) me = rr[r];
         int k = me.nonempty ? tid : -1, dummy = -1;
@@ -335,12 +411,17 @@ blocks_rowscan_kernel(BlocksParams P, RowRec *__restrict__ rows, FrameRec *__res
         FrameRec fr; fr.pad0 = fr.pad1 = 0;
         if (c_last < 0) { fr.size = 0; fr.trailing = 0; }                 // :390-395
         else {
-            fr.trailing = (uint32_t)(P.rows - 1 - c_last);
+            fr.trailing = (uint32_t)(g.rows() - 1 - c_last);
             fr.size = c_run + (fr.trailing ? 3 + ndig(fr.trailing) : 0);  // :397-399
         }
-        if (P.prev_mode == 3 && f == 0) { fr.size = 0; fr.trailing = 0; }   // halo frame of a sharded animation: reference only
+        if (g.prev_mode() == 3 && f == 0) { fr.size = 0; fr.trailing = 0; }   // halo frame of a sharded animation: reference only
         frames[f] = fr;
     }
+}
+
+__global__ void __launch_bounds__(BT)
+blocks_rowscan_kernel(BlocksParams P, RowRec *__restrict__ rows, FrameRec *__restrict__ frames) {
+    blocks_rowscan(UniformGeom(P, blockIdx.x, 0), rows, frames);
 }
 
 // Exclusive scan of a strided uint32 "size" field into uint64 offsets[n+1]; one block.
@@ -392,12 +473,13 @@ __device__ __forceinline__ char *put_color(char *o, uint32_t p, bool color8) {  
     o = put_u8s(o, p & 0xff); o = put_u8s(o, (p >> 8) & 0xff); return put_u8s(o, (p >> 16) & 0xff);
 }
 
-__global__ void __launch_bounds__(BT)
-blocks_emit_kernel(BlocksParams P, const CellRec *__restrict__ cells, const RowRec *__restrict__ rows,
-                   const FrameRec *__restrict__ frames, const uint64_t *__restrict__ offsets,
-                   char *__restrict__ out, unsigned long long out_cap) {
-    const int r = blockIdx.x, f = blockIdx.y, tid = threadIdx.x;
-    const RowRec rr = rows[(long long)f * P.rows + r];
+template <class G>
+__device__ __forceinline__ void blocks_emit(const G &g, bool color8, const CellRec *__restrict__ cells,
+                                            const RowRec *__restrict__ rows, const FrameRec *__restrict__ frames,
+                                            const uint64_t *__restrict__ offsets, char *__restrict__ out,
+                                            unsigned long long out_cap) {
+    const int r = g.r, f = g.f, tid = threadIdx.x;
+    const RowRec rr = rows[g.first_row_rec() + r];
     const FrameRec fr = frames[f];
     const unsigned long long fbase = offsets[f];
     if (fr.size == 0 || fbase + fr.size > out_cap) return; // nothing to write / never write out of bounds
@@ -412,9 +494,8 @@ blocks_emit_kernel(BlocksParams P, const CellRec *__restrict__ cells, const RowR
         char *o = rbase + yb + rr.len - 5;
         o[0] = '\033'; o[1] = '['; o[2] = '0'; o[3] = 'm'; o[4] = '\n';
     }
-    const CellRec *crow = cells + ((long long)f * P.rows + r) * P.cols;
-    const bool color8 = P.color8 != 0;
-    for (int c = tid; c < P.cols; c += BT) {
+    const CellRec *crow = cells + g.first_cell_rec();
+    for (int c = tid; c < g.cols(); c += BT) {
         const CellRec rec = crow[c];
         if (rec.meta & M_SKIPPED) continue;
         if (rec.meta & M_FIRST) {                          // pending y_skip, :249-258
@@ -449,6 +530,30 @@ blocks_emit_kernel(BlocksParams P, const CellRec *__restrict__ cells, const RowR
     }
 }
 
+__global__ void __launch_bounds__(BT)
+blocks_emit_kernel(BlocksParams P, const CellRec *__restrict__ cells, const RowRec *__restrict__ rows,
+                   const FrameRec *__restrict__ frames, const uint64_t *__restrict__ offsets,
+                   char *__restrict__ out, unsigned long long out_cap) {
+    blocks_emit(UniformGeom(P, blockIdx.y, blockIdx.x), P.color8 != 0, cells, rows, frames, offsets, out, out_cap);
+}
+
+// ---- mixed batches: one CTA per (frame, row pair) item of the flat list row_start describes (pick, emit), one per
+// frame (rowscan); frame f's items are row_start[f] .. row_start[f + 1] - 1
+__global__ void __launch_bounds__(BT)
+blocks_rowscan_mixed_kernel(const MixedBlocksFrame *__restrict__ desc, const unsigned *__restrict__ row_start,
+                            RowRec *__restrict__ rows, FrameRec *__restrict__ frames) {
+    blocks_rowscan(MixedGeom(desc, row_start, blockIdx.x, 0), rows, frames);
+}
+__global__ void __launch_bounds__(BT)
+blocks_emit_mixed_kernel(const MixedBlocksFrame *__restrict__ desc, const unsigned *__restrict__ row_start, int n_frames,
+                         int flags, const CellRec *__restrict__ cells, const RowRec *__restrict__ rows,
+                         const FrameRec *__restrict__ frames, const uint64_t *__restrict__ offsets,
+                         char *__restrict__ out, unsigned long long out_cap) {
+    const int f = mixed_owner(row_start, n_frames, blockIdx.x);
+    blocks_emit(MixedGeom(desc, row_start, f, (int)(blockIdx.x - row_start[f])), (flags & B200TIMG_COLOR8) != 0, cells, rows,
+                frames, offsets, out, out_cap);
+}
+
 int launch_blocks(b200timg_ctx *ctx, const uint8_t *d_fb, const uint8_t *d_prev, int prev_mode,
                   int w, int h, int n_frames, int flags, int x_indent, char *d_out,
                   size_t out_cap, uint64_t *d_offsets) {
@@ -479,7 +584,7 @@ int launch_blocks(b200timg_ctx *ctx, const uint8_t *d_fb, const uint8_t *d_prev,
 
     const dim3 grid(P.rows, n_frames);
     B2_KERNEL(ctx, "blocks_pick_kernel");
-    blocks_pick_kernel<<<grid, BT, 0, ctx->stream>>>(reinterpret_cast<const uint32_t *>(d_fb),
+    blocks_pick_kernel<UniformGeom><<<grid, BT, 0, ctx->stream>>>(reinterpret_cast<const uint32_t *>(d_fb),
                                                      reinterpret_cast<const uint32_t *>(d_prev), P, cells, rows);
     B2_LAUNCH_CHECK(ctx);
     B2_KERNEL(ctx, "blocks_rowscan_kernel");
@@ -492,6 +597,65 @@ int launch_blocks(b200timg_ctx *ctx, const uint8_t *d_fb, const uint8_t *d_prev,
     B2_KERNEL(ctx, "blocks_emit_kernel");
     blocks_emit_kernel<<<grid, BT, 0, ctx->stream>>>(P, cells, rows, frames, d_offsets, d_out,
                                                      (unsigned long long)out_cap);
+    B2_LAUNCH_CHECK(ctx);
+    return B200TIMG_OK;
+}
+
+// Block records of a mixed batch: frame f's scaled pixels follow the earlier frames' back to back (as
+// launch_scale_mixed writes them), its row and cell records follow the earlier frames' likewise.
+int plan_blocks_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *mb, MixedPlan &mp) {
+    const int n = mb->n_frames;
+    const bool quarter = (mb->flags & B200TIMG_QUARTER) != 0, upper = (mb->flags & B200TIMG_UPPER) != 0;
+    std::vector<MixedBlocksFrame> desc(n);
+    std::vector<unsigned> row_start(n + 1);
+    unsigned long long px = 0, cells = 0, rows = 0;
+    for (int f = 0; f < n; ++f) {
+        const b200timg_frame &F = mb->frames[f];
+        MixedBlocksFrame &D = desc[f];
+        D.fb_px = px; D.cell0 = cells;
+        D.w = F.out_w; D.h = F.out_h;
+        D.cols = quarter ? F.out_w / 2 : F.out_w;
+        D.rows = (F.out_h + 1) / 2;
+        D.row_offset = ((F.out_h & 1) && !upper) ? -1 : 0;
+        D.indent = F.x_indent_cells;
+        row_start[f] = (unsigned)rows;
+        px += (unsigned long long)F.out_w * F.out_h;
+        cells += (unsigned long long)D.rows * D.cols;
+        rows += (unsigned long long)D.rows;
+        if (rows > 0x7fffffffull)
+            return ctx->fail(B200TIMG_EINVAL, "mixed batch: more than 2^31 - 1 row pairs in one call (at frame %d)", f);
+    }
+    row_start[n] = (unsigned)rows;
+    mp.o_blocks = mixed_put(mp.arena, desc.data(), sizeof(MixedBlocksFrame) * n);
+    mp.o_rows = mixed_put(mp.arena, row_start.data(), sizeof(unsigned) * (n + 1));
+    mp.rowpairs = (unsigned)rows; mp.cells = cells;
+    return B200TIMG_OK;
+}
+
+int launch_blocks_mixed(b200timg_ctx *ctx, const MixedPlan &mp, const char *d_arena, const uint8_t *d_fb, int n_frames,
+                        int flags, char *d_out, size_t out_cap, uint64_t *d_offsets) {
+    B2_CUDA(ctx, ctx->cells.reserve((size_t)mp.cells * sizeof(CellRec)));
+    B2_CUDA(ctx, ctx->rows.reserve((size_t)mp.rowpairs * sizeof(RowRec) + (size_t)n_frames * sizeof(FrameRec) + 64));
+    CellRec *cells = ctx->cells.as<CellRec>();
+    RowRec *rows = ctx->rows.as<RowRec>();
+    FrameRec *frames = reinterpret_cast<FrameRec *>(rows + mp.rowpairs);
+    const MixedBlocksFrame *desc = reinterpret_cast<const MixedBlocksFrame *>(d_arena + mp.o_blocks);
+    const unsigned *row_start = reinterpret_cast<const unsigned *>(d_arena + mp.o_rows);
+    const uint32_t *fb = reinterpret_cast<const uint32_t *>(d_fb);
+    B2_KERNEL(ctx, "blocks_pick_mixed_kernel");
+    blocks_pick_kernel<MixedGeom><<<mp.rowpairs, BT, 0, ctx->stream>>>(fb, nullptr, MixedBlocksParams{desc, row_start, n_frames, flags},
+                                                                       cells, rows);
+    B2_LAUNCH_CHECK(ctx);
+    B2_KERNEL(ctx, "blocks_rowscan_mixed_kernel");
+    blocks_rowscan_mixed_kernel<<<n_frames, BT, 0, ctx->stream>>>(desc, row_start, rows, frames);
+    B2_LAUNCH_CHECK(ctx);
+    B2_KERNEL(ctx, "sizes_to_offsets_kernel");
+    sizes_to_offsets_kernel<<<1, 1024, 0, ctx->stream>>>(reinterpret_cast<const uint32_t *>(frames),
+                                                         sizeof(FrameRec) / 4, n_frames, d_offsets);
+    B2_LAUNCH_CHECK(ctx);
+    B2_KERNEL(ctx, "blocks_emit_mixed_kernel");
+    blocks_emit_mixed_kernel<<<mp.rowpairs, BT, 0, ctx->stream>>>(desc, row_start, n_frames, flags, cells, rows, frames,
+                                                                  d_offsets, d_out, (unsigned long long)out_cap);
     B2_LAUNCH_CHECK(ctx);
     return B200TIMG_OK;
 }

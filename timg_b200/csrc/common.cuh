@@ -119,6 +119,11 @@ struct b200timg_ctx {
     cudaEvent_t ev_gather_ready = nullptr, ev_gather_done[4] = {nullptr, nullptr, nullptr, nullptr};
     uint64_t gather_seq = 0;
     b200timg::DevBuf gather_status;
+    // mixed batches (b200timg_mixed_batch): the call's tables and descriptors, uploaded in one copy from mixed_stage;
+    // the staging is rewritten only once ev_mixed says the previous call's copy has run
+    b200timg::DevBuf mixed_arena;
+    b200timg::HostBuf mixed_stage;
+    cudaEvent_t ev_mixed = nullptr;
 
     int fail(int code, const char *fmt, ...) {
         va_list ap; va_start(ap, fmt);
@@ -267,5 +272,40 @@ int launch_deflate_pack(b200timg_ctx *ctx, const uint8_t *d_raw, long long raw_s
                         const uint8_t *d_scratch, const DeflateSeg *d_info, const unsigned long long *d_start, uint8_t *d_png,
                         long long png_stride, int zoff);
 int sixel_debug_fetch(b200timg_ctx *ctx, uint32_t *h_palette, uint32_t *h_counts, uint8_t *h_index, size_t index_bytes);
+
+// ---- mixed batches (b200timg_mixed_batch) ----------------------------------------------------------------------
+// One frame of a mixed batch as the block encoder sees it (blocks.cu).
+struct __align__(16) MixedBlocksFrame {
+    unsigned long long fb_px;    // first pixel of the scaled frame, in pixels from the batch's framebuffer
+    unsigned long long cell0;    // first cell record
+    int w, h, cols, rows, row_offset, indent;
+};
+// Everything the kernels of one mixed call read that the host computes, built once per call and uploaded in one copy
+// to ctx->mixed_arena: the scaler's tables and frame descriptors (plan_scale_mixed, resample.cu) and the block
+// encoder's (plan_blocks_mixed, blocks.cu).
+struct MixedPlan {
+    std::vector<char> arena;                       // host image of the upload
+    size_t o_scale = 0, o_p1 = 0, o_p2 = 0, o_tab = 0, o_blocks = 0, o_rows = 0;   // byte offsets of its parts
+    std::vector<unsigned> p1, p2;                  // [n+1] first CTA of each frame in the scaler's two passes
+    std::vector<int> group_end;                    // scaler frame groups: frames [previous end, end)
+    size_t tmp_elems = 0;                          // float4 intermediate of the largest group
+    unsigned long long out_px = 0;                 // scaled pixels of the whole batch
+    unsigned rowpairs = 0;                         // block encoder: (frame, row pair) items ...
+    unsigned long long cells = 0;                  // ... and cell records
+};
+// appends bytes at a 16-byte boundary of the arena and returns their offset
+inline size_t mixed_put(std::vector<char> &a, const void *p, size_t bytes) {
+    const size_t o = (a.size() + 15) / 16 * 16;
+    a.resize(o + bytes);
+    if (bytes) memcpy(a.data() + o, p, bytes);
+    return o;
+}
+int plan_scale_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *b, MixedPlan &mp);
+int plan_blocks_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *b, MixedPlan &mp);
+// scale + fused compose of every frame into d_out (frames back to back)
+int launch_scale_mixed(b200timg_ctx *ctx, const MixedPlan &mp, const char *d_arena, const uint8_t *d_src, uint8_t *d_out,
+                       int n_frames, int bgra, const ComposeSpec &cs);
+int launch_blocks_mixed(b200timg_ctx *ctx, const MixedPlan &mp, const char *d_arena, const uint8_t *d_fb, int n_frames,
+                        int flags, char *d_out, size_t out_cap, uint64_t *d_offsets);
 
 }  // namespace b200timg

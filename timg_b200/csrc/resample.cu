@@ -10,6 +10,8 @@
 // working set of a tile stays in L1/L2).  Algorithmic bytes: 4*iw*ih read + 4*ow*oh written.
 #include <algorithm>
 #include <cstdlib>
+#include <map>
+#include <tuple>
 #include <type_traits>
 #include <vector>
 
@@ -1689,6 +1691,248 @@ int launch_scale(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int fmt
         }
     }
     B2_LAUNCH_CHECK(ctx);
+    return B200TIMG_OK;
+}
+
+// ---- mixed-geometry batches (b200timg_mixed_batch) ---------------------------------------------------------------
+// Frames of different geometry in a fixed number of launches: the two 1-D passes of the twopass_* kernels (same
+// decode, tap order, accumulators, un-weighting and encode), each over a flat list of (frame, CTA) items so that one
+// launch covers every frame whatever its geometry and tap count.  Frame f's pass-p CTAs are p_start[f] ..
+// p_start[f + 1] - 1 and each covers 256 consecutive elements of the frame's pass output, row-major:
+//   pass 1  the first axis of the frame's plan, into a float4 intermediate (vertical first: oh x iw; else ih x ow);
+//   pass 2  the other axis, un-weight, encode, compose (or the plain copy of a copy_only frame).
+// Transparency follows the twopass scheme: pixels whose filtered alpha is below 2^-120 raise their frame's flag and are
+// filled in by a second pair of passes on the un-weighted colour planes (which returns at once for opaque frames).
+struct __align__(16) MixedScaleFrame {
+    unsigned long long src_off;    // bytes from the batch's source
+    unsigned long long out_px;     // first output pixel (and mask byte), in pixels from the batch's output
+    unsigned long long tmp_off;    // first intermediate element, in float4 from the group's intermediate
+    unsigned long long tab;        // this geometry's tables, in 4-byte words from the table arena:
+                                   // h_first[ow] h_count[ow] v_first[oh] v_count[oh] h_coeff[ow][hw] v_coeff[oh][vw]
+    int iw, ih, ow, oh, h_widest, v_widest, vertical_first, h_sequential, copy_only;
+};
+
+// frame that owns flat item b: the last f with start[f] <= b (frames without items share their start)
+__device__ __forceinline__ int mixed_frame_of(const unsigned *__restrict__ start, int n, unsigned b) {
+    int lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (start[mid] <= b) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+// horizontal taps as twopass_h1_kernel / twopass_2_kernel sum them; ld(i) is tap i's float4
+template <class Load>
+__device__ __forceinline__ float4 mixed_hsum(Load ld, const float *hc, int cnt, bool sequential) {
+    if (sequential) {
+        float4 r = mul4(ld(0), hc[0]);
+        for (int i = 1; i < cnt; ++i) r = add4(r, mul4(ld(i), hc[i]));
+        return r;
+    }
+    const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+    float4 a0 = z, a1 = z;
+    for (int i = 0; i < cnt; ++i) { const float4 t = mul4(ld(i), hc[i]); if (i & 1) a1 = add4(a1, t); else a0 = add4(a0, t); }
+    return add4(a0, a1);
+}
+// vertical taps in input-row order, as twopass_v1_kernel / twopass_2_kernel
+template <class Load>
+__device__ __forceinline__ float4 mixed_vsum(Load ld, const float *vc, int cnt) {
+    float4 a = mul4(ld(0), vc[0]);
+    for (int k = 1; k < cnt; ++k) a = add4(a, mul4(ld(k), vc[k]));
+    return a;
+}
+
+struct MixedScaleArgs {
+    const uint8_t *src;
+    const MixedScaleFrame *frames;
+    const unsigned *start;         // p1 or p2 of the plan
+    const int32_t *tab;
+    float4 *tmp;
+    int *need_plain;               // [n_frames]
+    unsigned char *mask;           // [output pixels] 1 = filtered alpha < 2^-120
+    uint32_t *out;
+    int n_frames, bgra;
+    unsigned b0, b1;               // this launch covers items b0 .. b1 - 1
+    ComposeSpec cs;
+};
+
+template <bool PLAIN>
+__global__ void __launch_bounds__(256)
+mixed_pass1_kernel(MixedScaleArgs A) {
+    const unsigned b = A.b0 + blockIdx.x;
+    if (b >= A.b1) return;
+    const int f = mixed_frame_of(A.start, A.n_frames, b);
+    if (PLAIN && !A.need_plain[f]) return;
+    const MixedScaleFrame F = A.frames[f];
+    const long long e = (long long)(b - A.start[f]) * 256 + threadIdx.x;
+    const uint32_t *in = reinterpret_cast<const uint32_t *>(A.src + F.src_off);
+    const int32_t *h_first = A.tab + F.tab, *h_count = h_first + F.ow, *v_first = h_count + F.ow, *v_count = v_first + F.oh;
+    const float *h_coeff = reinterpret_cast<const float *>(v_count + F.oh), *v_coeff = h_coeff + (long long)F.ow * F.h_widest;
+    const int bgra = A.bgra;
+    float4 r;
+    if (F.vertical_first) {                       // tmp[oy][x] = sum_k decode(src[v_first[oy] + k][x]) * vc[oy][k]
+        if (e >= (long long)F.oh * F.iw) return;
+        const int oy = (int)(e / F.iw), x = (int)(e - (long long)oy * F.iw);
+        const uint32_t *col = in + (long long)v_first[oy] * F.iw + x;
+        const int iw = F.iw;
+        r = mixed_vsum([&](int k) { return decode_tp<PLAIN>(col[(long long)k * iw], bgra); },
+                       v_coeff + (long long)oy * F.v_widest, v_count[oy]);
+    } else {                                      // tmp[y][ox] = sum_i decode(src[y][h_first[ox] + i]) * hc[ox][i]
+        if (e >= (long long)F.ih * F.ow) return;
+        const int y = (int)(e / F.ow), ox = (int)(e - (long long)y * F.ow);
+        const uint32_t *row = in + (long long)y * F.iw + h_first[ox];
+        r = mixed_hsum([&](int i) { return decode_tp<PLAIN>(row[i], bgra); }, h_coeff + (long long)ox * F.h_widest,
+                       h_count[ox], F.h_sequential != 0);
+    }
+    A.tmp[F.tmp_off + e] = r;
+}
+
+template <bool PLAIN>
+__global__ void __launch_bounds__(256)
+mixed_pass2_kernel(MixedScaleArgs A) {
+    const unsigned b = A.b0 + blockIdx.x;
+    if (b >= A.b1) return;
+    const int f = mixed_frame_of(A.start, A.n_frames, b);
+    if (PLAIN && !A.need_plain[f]) return;
+    const MixedScaleFrame F = A.frames[f];
+    const long long e = (long long)(b - A.start[f]) * 256 + threadIdx.x;
+    if (e >= (long long)F.ow * F.oh) return;
+    const int oy = (int)(e / F.ow), ox = (int)(e - (long long)oy * F.ow);
+    const int32_t *h_first = A.tab + F.tab, *h_count = h_first + F.ow, *v_first = h_count + F.ow, *v_count = v_first + F.oh;
+    const float *h_coeff = reinterpret_cast<const float *>(v_count + F.oh), *v_coeff = h_coeff + (long long)F.ow * F.h_widest;
+    uint32_t *dst = A.out + F.out_px + e;
+    if (F.copy_only) {                            // both axes point-sampled, as resample_copy_kernel
+        if (PLAIN) return;
+        uint32_t p = reinterpret_cast<const uint32_t *>(A.src + F.src_off)[(long long)v_first[oy] * F.iw + h_first[ox]];
+        if (A.bgra) p = (p & 0xff00ff00u) | ((p & 0xff) << 16) | ((p >> 16) & 0xff);
+        *dst = compose_at(A.cs, p, ox, oy);
+        return;
+    }
+    const float4 *tmp = A.tmp + F.tmp_off;
+    float4 r;
+    if (F.vertical_first) {                       // second pass is horizontal, over tmp[oy][0..iw)
+        const float4 *row = tmp + (long long)oy * F.iw + h_first[ox];
+        r = mixed_hsum([&](int i) { return row[i]; }, h_coeff + (long long)ox * F.h_widest, h_count[ox], F.h_sequential != 0);
+    } else {                                      // second pass is vertical, over tmp[0..ih)[ox]
+        const float4 *col = tmp + (long long)v_first[oy] * F.ow + ox;
+        const int ow = F.ow;
+        r = mixed_vsum([&](int k) { return col[(long long)k * ow]; }, v_coeff + (long long)oy * F.v_widest, v_count[oy]);
+    }
+    const float tiny = 7.5231638452626401e-37f;   // 2^-120
+    float v[7];
+    unsigned char *m = A.mask + F.out_px + e;
+    if (!PLAIN) {
+        const bool hole = r.w < tiny;             // un-weighted colour needed: left to the plain passes
+        *m = hole ? 1 : 0;
+        if (hole) { A.need_plain[f] = 1; return; }
+        v[0] = v[1] = v[2] = 0.f; v[3] = r.w; v[4] = r.x; v[5] = r.y; v[6] = r.z;
+        *dst = compose_at(A.cs, encode_px(v), ox, oy);
+    } else if (*m) {
+        v[0] = r.x; v[1] = r.y; v[2] = r.z; v[3] = 0.f; v[4] = v[5] = v[6] = 0.f;
+        *dst = compose_at(A.cs, encode_px(v), ox, oy);
+    }
+}
+
+// Tables and descriptors of every frame; frames of equal geometry share one plan.  Frame groups bound the float
+// intermediate: a group closes before the frame that would take it past the budget (a frame alone may exceed it).
+int plan_scale_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *mb, MixedPlan &mp) {
+    const int n = mb->n_frames;
+    unsigned long long budget = 2ull << 30;
+    if (const char *e = getenv("B200TIMG_MIXED_GROUP_BYTES")) budget = std::max(1ull, strtoull(e, nullptr, 10));   // test knob
+    std::vector<MixedScaleFrame> desc(n);
+    std::vector<int32_t> tab;
+    struct Geom { int iw, ih, ow, oh; unsigned long long tab; int hw, vw, vertical_first, h_sequential, copy_only; };
+    std::vector<Geom> geoms;
+    std::map<std::tuple<int, int, int, int>, size_t> index;     // geometry -> its entry in geoms
+    mp.p1.assign(n + 1, 0); mp.p2.assign(n + 1, 0);
+    mp.group_end.clear();
+    unsigned long long p1 = 0, p2 = 0, out_px = 0, group_tmp = 0;
+    ResamplePlan pl;
+    for (int f = 0; f < n; ++f) {
+        const b200timg_frame &F = mb->frames[f];
+        MixedScaleFrame &D = desc[f];
+        const auto key = std::make_tuple(F.src_w, F.src_h, F.out_w, F.out_h);
+        const auto hit = index.find(key);
+        const size_t g = hit != index.end() ? hit->second : geoms.size();
+        if (g == geoms.size()) {
+            index.emplace(key, g);
+            if (!build_resample_plan(F.src_w, F.src_h, F.out_w, F.out_h, &pl))
+                return ctx->fail(B200TIMG_EINVAL, "mixed batch: frame %d: degenerate geometry %dx%d -> %dx%d", f, F.src_w, F.src_h,
+                                 F.out_w, F.out_h);
+            geoms.push_back({F.src_w, F.src_h, F.out_w, F.out_h, tab.size(), pl.h.widest, pl.v.widest, pl.vertical_first ? 1 : 0,
+                             pl.h_sequential ? 1 : 0, pl.copy_only ? 1 : 0});
+            auto put = [&](const void *p, size_t words) { const int32_t *w = static_cast<const int32_t *>(p); tab.insert(tab.end(), w, w + words); };
+            put(pl.h.first.data(), F.out_w); put(pl.h.count.data(), F.out_w);
+            put(pl.v.first.data(), F.out_h); put(pl.v.count.data(), F.out_h);
+            put(pl.h.coeff.data(), pl.h.coeff.size()); put(pl.v.coeff.data(), pl.v.coeff.size());
+        }
+        const Geom &G = geoms[g];
+        D.src_off = F.src_offset;
+        D.out_px = out_px;
+        D.tab = G.tab;
+        D.iw = F.src_w; D.ih = F.src_h; D.ow = F.out_w; D.oh = F.out_h;
+        D.h_widest = G.hw; D.v_widest = G.vw;
+        D.vertical_first = G.vertical_first; D.h_sequential = G.h_sequential; D.copy_only = G.copy_only;
+        const unsigned long long elems = D.copy_only ? 0ull
+                                       : D.vertical_first ? (unsigned long long)F.out_h * F.src_w : (unsigned long long)F.src_h * F.out_w;
+        if (group_tmp && (group_tmp + elems) * sizeof(float4) > budget) { mp.group_end.push_back(f); group_tmp = 0; }
+        D.tmp_off = group_tmp;
+        group_tmp += elems;
+        mp.tmp_elems = std::max<size_t>(mp.tmp_elems, (size_t)group_tmp);
+        mp.p1[f] = (unsigned)p1; mp.p2[f] = (unsigned)p2;
+        p1 += (elems + 255) / 256;
+        p2 += ((unsigned long long)F.out_w * F.out_h + 255) / 256;
+        out_px += (unsigned long long)F.out_w * F.out_h;
+        if (p1 > 0x7fffffffull || p2 > 0x7fffffffull)
+            return ctx->fail(B200TIMG_EINVAL, "mixed batch: more than 2^31 - 1 scaler work items in one call (at frame %d)", f);
+    }
+    mp.group_end.push_back(n);
+    mp.p1[n] = (unsigned)p1; mp.p2[n] = (unsigned)p2;
+    mp.out_px = out_px;
+    mp.o_scale = mixed_put(mp.arena, desc.data(), sizeof(MixedScaleFrame) * n);
+    mp.o_p1 = mixed_put(mp.arena, mp.p1.data(), sizeof(unsigned) * (n + 1));
+    mp.o_p2 = mixed_put(mp.arena, mp.p2.data(), sizeof(unsigned) * (n + 1));
+    mp.o_tab = mixed_put(mp.arena, tab.data(), sizeof(int32_t) * tab.size());
+    return B200TIMG_OK;
+}
+
+int launch_scale_mixed(b200timg_ctx *ctx, const MixedPlan &mp, const char *d_arena, const uint8_t *d_src, uint8_t *d_out,
+                       int n_frames, int bgra, const ComposeSpec &cs) {
+    // scratch: [intermediate of the largest group | need_plain per frame | mask per output pixel]
+    const size_t o_flag = (sizeof(float4) * std::max<size_t>(1, mp.tmp_elems) + 255) / 256 * 256;
+    const size_t o_mask = o_flag + (sizeof(int) * (size_t)n_frames + 255) / 256 * 256;
+    B2_CUDA(ctx, ctx->scale_tmp.reserve(o_mask + (size_t)mp.out_px));
+    char *tb = ctx->scale_tmp.as<char>();
+    MixedScaleArgs A;
+    A.src = d_src;
+    A.frames = reinterpret_cast<const MixedScaleFrame *>(d_arena + mp.o_scale);
+    A.tab = reinterpret_cast<const int32_t *>(d_arena + mp.o_tab);
+    A.tmp = reinterpret_cast<float4 *>(tb);
+    A.need_plain = reinterpret_cast<int *>(tb + o_flag);
+    A.mask = reinterpret_cast<unsigned char *>(tb + o_mask);
+    A.out = reinterpret_cast<uint32_t *>(d_out);
+    A.n_frames = n_frames; A.bgra = bgra; A.cs = cs;
+    B2_CUDA(ctx, cudaMemsetAsync(A.need_plain, 0, sizeof(int) * (size_t)n_frames, ctx->stream));
+    int f0 = 0;
+    for (const int f1 : mp.group_end) {
+        for (int plain = 0; plain < 2; ++plain) {
+            // a group without pass-1 work (copy_only frames only) still launches one CTA, so that the number of
+            // launches depends on the group count alone
+            A.start = reinterpret_cast<const unsigned *>(d_arena + mp.o_p1);
+            A.b0 = mp.p1[f0]; A.b1 = mp.p1[f1];
+            B2_KERNEL(ctx, plain ? "mixed_plain_kernels" : "mixed_pass1_kernel");
+            if (plain) mixed_pass1_kernel<true><<<std::max(1u, A.b1 - A.b0), 256, 0, ctx->stream>>>(A);
+            else mixed_pass1_kernel<false><<<std::max(1u, A.b1 - A.b0), 256, 0, ctx->stream>>>(A);
+            B2_LAUNCH_CHECK(ctx);
+            A.start = reinterpret_cast<const unsigned *>(d_arena + mp.o_p2);
+            A.b0 = mp.p2[f0]; A.b1 = mp.p2[f1];
+            B2_KERNEL(ctx, plain ? "mixed_plain_kernels" : "mixed_pass2_kernel");
+            if (plain) mixed_pass2_kernel<true><<<std::max(1u, A.b1 - A.b0), 256, 0, ctx->stream>>>(A);
+            else mixed_pass2_kernel<false><<<std::max(1u, A.b1 - A.b0), 256, 0, ctx->stream>>>(A);
+            B2_LAUNCH_CHECK(ctx);
+        }
+        f0 = f1;
+    }
     return B200TIMG_OK;
 }
 

@@ -1,0 +1,271 @@
+#!/usr/bin/env python
+"""Mixed batches on the GPU: a `timg --grid` page of differently sized images, block-encoded in one call
+(b200timg_blocks_mixed_dev) against the ways to send it without one.  One JSON line per page.
+
+  python tools/bench_mixed.py [--steps K] [--warmup W] [--only NAME]
+
+  grid8x8-quarter  --grid=8x8 -g300x100 -p quarter: 64 images, each fitted to the grid's 75 x 25 px box
+  grid4x4-half     --grid=4x4 -g300x100 -p half: 16 images fitted to 75 x 50 px (larger outputs per image)
+Source sizes cycle through 3840x2160, 2160x3840, 4032x3024, 3000x2000, 1920x1080, 1280x720, 1080x1080 and 640x480
+(every image's pixels distinct); indents are the renderer's column offsets (src/renderer.cc:124-142).
+
+Timed, alternating within each step, every call ending in a device-wide synchronise:
+  (a) mixed     one b200timg_blocks_mixed_dev call for the page
+  (b) per_image one b200timg_blocks_batch_dev call per image (n_frames = 1): the status quo
+  (c) per_geom  one uniform b200timg_blocks_batch_dev call per distinct geometry (sources regrouped by geometry)
+  (d) the cost of generality: C3 geometry (1920x1080 -> 320x90, -p quarter, 64 frames) through the mixed call against
+      b200timg_blocks_batch_dev
+(a), (b) and (c) must produce the same bytes for every image (asserted); so must both sides of (d).  Per-kernel ms of one
+(a) and one (b) page come from b200timg_profile in a separate run.  The GPU's name, power limit and max SM clock are read
+in the same run.
+"""
+import argparse
+import ctypes as C
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+import timg_b200  # noqa: E402
+from timg_b200 import synth  # noqa: E402
+
+SIZES = [(3840, 2160), (2160, 3840), (4032, 3024), (3000, 2000), (1920, 1080), (1280, 720), (1080, 1080), (640, 480)]
+PAGES = {
+    "grid8x8-quarter": dict(cols=8, rows=8, term=(300, 100), quarter=True),
+    "grid4x4-half": dict(cols=4, rows=4, term=(300, 100), quarter=False),
+}
+
+
+def gpu_info():
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30)
+        return r.stdout.strip().splitlines()[0]
+    except Exception as e:                      # the numbers still stand, without their card
+        return f"unavailable ({e})"
+
+
+def page_layout(cfg):
+    """(images' source sizes, fitted outputs, indents) of one page, as timg.cc:938-939 and renderer.cc lay it out."""
+    cx, cy = (2, 2) if cfg["quarter"] else (1, 2)
+    box_w = cfg["term"][0] * cx // cfg["cols"]
+    box_h = cfg["term"][1] * cy // cfg["rows"]
+    n = cfg["cols"] * cfg["rows"]
+    srcs, outs, indents = [], [], []
+    for i in range(n):
+        iw, ih = SIZES[i % len(SIZES)]
+        _, ow, oh = timg_b200.calc_fit(iw, ih, box_w, box_h, cx, cy)
+        srcs.append((iw, ih))
+        outs.append((ow, oh))
+        indents.append((i % cfg["cols"]) * box_w // cx)     # UnicodeBlockCanvas::Send's x / cell_x_px
+    return srcs, outs, indents
+
+
+def device_images(torch, srcs):
+    """One generated base image per size; image i is its base with a per-image byte rotation of the colours."""
+    base = {s: synth.frame_torch(700 + k, s[0], s[1], "photo") for k, s in enumerate(SIZES)}
+    imgs = []
+    for i, s in enumerate(srcs):
+        im = base[s].clone()
+        im[..., :3] += (29 * (i // len(SIZES)) + 1) & 255
+        imgs.append(im)
+    return imgs
+
+
+def pack(torch, imgs):
+    sizes = [im.numel() for im in imgs]
+    offs = np.cumsum([0] + sizes)
+    flat = torch.empty(int(offs[-1]), dtype=torch.uint8, device="cuda")
+    for im, o in zip(imgs, offs):
+        flat[int(o):int(o) + im.numel()] = im.reshape(-1)
+    return flat, [int(o) for o in offs[:-1]]
+
+
+def timed(torch, fn, steps):
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    for _ in range(steps):
+        fn()
+    torch.cuda.synchronize()
+    return (time.perf_counter() - t0) * 1e3 / steps
+
+
+def run_page(name, cfg, steps, warmup, torch):
+    L = timg_b200.lib()
+    ctx = timg_b200.Context(0)
+    flags = timg_b200.QUARTER if cfg["quarter"] else 0
+    bg = timg_b200.rgba_u32(0, 0, 0)
+    srcs, outs, indents = page_layout(cfg)
+    n = len(srcs)
+    imgs = device_images(torch, srcs)
+    flat, offs = pack(torch, imgs)
+    torch.cuda.synchronize()                   # sources are written on torch's stream, read on the context's
+    mb, keep = timg_b200.mixed_batch([(h, w) for w, h in srcs], outs, offs, indents, flags, has_bg=True, bg=bg)
+    bounds = [L.b200timg_blocks_bound(ow, oh) for ow, oh in outs]
+    cap = sum(bounds)
+    d_out_a = torch.empty(cap, dtype=torch.uint8, device="cuda")
+    d_offs_a = torch.empty(n + 1, dtype=torch.int64, device="cuda")
+
+    def batch(iw, ih, ow, oh, nf, indent):
+        return timg_b200.Batch(n_frames=nf, src_w=iw, src_h=ih, src_fmt=0, out_w=ow, out_h=oh, has_bg=1, bg=bg, pattern=0,
+                               pattern_w=0, pattern_h=0, flags=flags, x_indent_cells=indent, animation=0)
+
+    def run_a():
+        ctx._chk(L.b200timg_blocks_mixed_dev(ctx.h, C.byref(mb), flat.data_ptr(), d_out_a.data_ptr(), cap, d_offs_a.data_ptr()))
+
+    # (b): one call per image, image i's bytes in its own slot
+    slot = np.cumsum([0] + bounds)
+    d_out_b = torch.empty(cap, dtype=torch.uint8, device="cuda")
+    d_offs_b = torch.empty((n, 2), dtype=torch.int64, device="cuda")
+    b_batches = [batch(srcs[i][0], srcs[i][1], outs[i][0], outs[i][1], 1, indents[i]) for i in range(n)]
+
+    def run_b():
+        for i in range(n):
+            ctx._chk(L.b200timg_blocks_batch_dev(ctx.h, C.byref(b_batches[i]), flat.data_ptr() + offs[i],
+                                                 d_out_b.data_ptr() + int(slot[i]), bounds[i], d_offs_b[i].data_ptr()))
+
+    # (c): images regrouped by geometry; one uniform call per geometry (the indent is per call, so frames of a group
+    # that sit in different columns would need one call each: the bytes are compared with indents folded in below)
+    geoms = {}
+    for i in range(n):
+        geoms.setdefault((srcs[i], outs[i], indents[i]), []).append(i)
+    order = [i for g in geoms.values() for i in g]
+    flat_c, offs_c = pack(torch, [imgs[i] for i in order])
+    torch.cuda.synchronize()
+    d_out_c = torch.empty(cap, dtype=torch.uint8, device="cuda")
+    c_calls, pos = [], 0
+    for (src, out, indent), members in geoms.items():
+        k = len(members)
+        gcap = k * L.b200timg_blocks_bound(*out)
+        c_calls.append((batch(src[0], src[1], out[0], out[1], k, indent), offs_c[pos], gcap,
+                        torch.empty(k + 1, dtype=torch.int64, device="cuda"), members))
+        pos += k
+    c_base = np.cumsum([0] + [c[2] for c in c_calls])
+
+    def run_c():
+        for j, (b, o, gcap, d_o, _) in enumerate(c_calls):
+            ctx._chk(L.b200timg_blocks_batch_dev(ctx.h, C.byref(b), flat_c.data_ptr() + o, d_out_c.data_ptr() + int(c_base[j]),
+                                                 gcap, d_o.data_ptr()))
+
+    for _ in range(warmup):
+        run_a(); run_b(); run_c()
+    torch.cuda.synchronize()
+    t = {"a": 0.0, "b": 0.0, "c": 0.0}
+    for _ in range(steps):                     # alternating, one page each
+        t["a"] += timed(torch, run_a, 1)
+        t["b"] += timed(torch, run_b, 1)
+        t["c"] += timed(torch, run_c, 1)
+    t = {k: v / steps for k, v in t.items()}
+
+    # same bytes, image by image
+    oa, da = d_offs_a.cpu().numpy(), d_out_a.cpu().numpy()
+    ob, db = d_offs_b.cpu().numpy(), d_out_b.cpu().numpy()
+    dc = d_out_c.cpu().numpy()
+    got_a = [da[oa[i]:oa[i + 1]].tobytes() for i in range(n)]
+    got_b = [db[int(slot[i]) + ob[i][0]:int(slot[i]) + ob[i][1]].tobytes() for i in range(n)]
+    got_c = [None] * n
+    for j, (_, _, _, d_o, members) in enumerate(c_calls):
+        oc = d_o.cpu().numpy()
+        for k, i in enumerate(members):
+            got_c[i] = dc[int(c_base[j]) + oc[k]:int(c_base[j]) + oc[k + 1]].tobytes()
+    assert got_a == got_b, "mixed call differs from per-image calls"
+    assert got_a == got_c, "mixed call differs from per-geometry calls"
+
+    kernels = {}
+    for key, fn in (("a", run_a), ("b", run_b)):
+        ctx.profile(True)
+        fn()
+        kernels[key] = {k: [v[0], round(v[1], 4)] for k, v in ctx.profile_report().items()}
+        ctx.profile(False)
+    src_px = sum(w * h for w, h in srcs)
+    res = dict(page=name, images=n, distinct_geometries=len({(s, o) for s, o in zip(srcs, outs)}), uniform_calls_c=len(c_calls),
+               outs=sorted({f"{o[0]}x{o[1]}" for o in outs}), src_mpx=round(src_px / 1e6, 1), encoded_bytes=int(oa[-1]),
+               steps=steps, same_bytes=True)
+    for k, label in (("a", "mixed"), ("b", "per_image"), ("c", "per_geom")):
+        res[f"{label}_ms"] = round(t[k], 3)
+        res[f"{label}_mpx_s"] = round(src_px / t[k] / 1e3, 1)
+    res["per_image_over_mixed"] = round(t["b"] / t["a"], 2)
+    res["per_geom_over_mixed"] = round(t["c"] / t["a"], 2)
+    res["kernels_ms_mixed"] = kernels["a"]
+    res["kernels_ms_per_image"] = kernels["b"]
+    ctx.close()
+    return res
+
+
+def run_generality(steps, warmup, torch):
+    """(d): C3 geometry through the mixed call and through the uniform batch."""
+    L = timg_b200.lib()
+    ctx = timg_b200.Context(0)
+    n, iw, ih, ow, oh, indent = 64, 1920, 1080, 320, 90, 0
+    bg = timg_b200.rgba_u32(0, 0, 0)
+    base = synth.frame_torch(800, iw, ih, "photo")
+    d_src = torch.empty((n, ih, iw, 4), dtype=torch.uint8, device="cuda")
+    for f in range(n):
+        d_src[f] = base
+        d_src[f, ..., :3] += (37 * f + 1) & 255
+    fbytes = iw * ih * 4
+    mb, keep = timg_b200.mixed_batch([(ih, iw)] * n, [(ow, oh)] * n, [f * fbytes for f in range(n)], [indent] * n,
+                                     timg_b200.QUARTER, has_bg=True, bg=bg)
+    ub = timg_b200.Batch(n_frames=n, src_w=iw, src_h=ih, src_fmt=0, out_w=ow, out_h=oh, has_bg=1, bg=bg, pattern=0, pattern_w=0,
+                         pattern_h=0, flags=timg_b200.QUARTER, x_indent_cells=indent, animation=0)
+    cap = n * L.b200timg_blocks_bound(ow, oh)
+    outs = [torch.empty(cap, dtype=torch.uint8, device="cuda") for _ in range(2)]
+    offs = [torch.empty(n + 1, dtype=torch.int64, device="cuda") for _ in range(2)]
+    torch.cuda.synchronize()
+
+    def mixed():
+        ctx._chk(L.b200timg_blocks_mixed_dev(ctx.h, C.byref(mb), d_src.data_ptr(), outs[0].data_ptr(), cap, offs[0].data_ptr()))
+
+    def uniform():
+        ctx._chk(L.b200timg_blocks_batch_dev(ctx.h, C.byref(ub), d_src.data_ptr(), outs[1].data_ptr(), cap, offs[1].data_ptr()))
+    for _ in range(warmup):
+        mixed(); uniform()
+    tm = tu = 0.0
+    for _ in range(steps):
+        tm += timed(torch, mixed, 1)
+        tu += timed(torch, uniform, 1)
+    tm, tu = tm / steps, tu / steps
+    same = bool((offs[0] == offs[1]).all()) and bool((outs[0][:int(offs[0][-1])] == outs[1][:int(offs[1][-1])]).all())
+    assert same, "mixed call differs from the uniform batch on C3 geometry"
+    kernels = {}
+    for key, fn in (("mixed", mixed), ("uniform", uniform)):
+        ctx.profile(True)
+        fn()
+        kernels[key] = {k: [v[0], round(v[1], 4)] for k, v in ctx.profile_report().items()}
+        ctx.profile(False)
+    ctx.close()
+    return dict(page="C3-generality", frames=n, src=f"{iw}x{ih}", out=f"{ow}x{oh}", steps=steps, same_bytes=same,
+                mixed_ms=round(tm, 3), uniform_ms=round(tu, 3), mixed_over_uniform=round(tm / tu, 2),
+                mixed_mpx_s=round(n * iw * ih / tm / 1e3, 1), uniform_mpx_s=round(n * iw * ih / tu / 1e3, 1),
+                kernels_ms_mixed=kernels["mixed"], kernels_ms_uniform=kernels["uniform"])
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--only", default=None)
+    a = ap.parse_args()
+    import torch
+    info = gpu_info()
+    for name, cfg in PAGES.items():
+        if a.only and a.only != name:
+            continue
+        r = run_page(name, cfg, a.steps, a.warmup, torch)
+        r["gpu"] = info
+        print(json.dumps(r), flush=True)
+        torch.cuda.empty_cache()
+    if not a.only or a.only == "C3-generality":
+        r = run_generality(a.steps, a.warmup, torch)
+        r["gpu"] = info
+        print(json.dumps(r), flush=True)
+
+
+if __name__ == "__main__":
+    main()
