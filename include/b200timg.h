@@ -249,7 +249,8 @@ int b200timg_sixel_batch(b200timg_ctx *ctx, const b200timg_batch *b, const uint8
  * unknown src_fmt, B200TIMG_BILINEAR_SCALE, more than 2^31 - 1 row pairs or scaler work items in one call.
  * B200TIMG_FAST_SCALE is accepted and ignored: mixed batches always scale bit-exactly.
  * Out of scope: delta frames (a grid page has none, so there is no animation field), YUV sources, the bilinear
- * scaler, and the sixel / kitty / iTerm2 encoders (they build on b200timg_scale_mixed_dev's output). */
+ * scaler, and the kitty / iTerm2 encoders (they build on b200timg_scale_mixed_dev's output).  The sixel encoder takes
+ * mixed batches: b200timg_sixel_mixed_dev below. */
 typedef struct {
     uint64_t src_offset;        /* bytes from the batch's source pointer to this frame's first pixel; multiple of 4 */
     int src_w, src_h;           /* source geometry of this image */
@@ -278,6 +279,21 @@ int b200timg_blocks_mixed_dev(b200timg_ctx *ctx, const b200timg_mixed_batch *b, 
                               char *d_out, size_t out_cap, uint64_t *d_offsets);
 int b200timg_blocks_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *b, const uint8_t *src,
                           char *out, size_t out_cap, uint64_t *offsets);
+/* scale -> compose -> pad -> sixel (a `-p sixel` grid page): frame f's bytes are exactly those of b200timg_sixel_batch_dev
+ * on a one-frame batch of that image with flags = 0 -- exact scale with the compose fused, padded to a multiple of 6
+ * rows, the background composed into the pad strip only (SixelCanvas::Send), palette, Floyd-Steinberg dither, DCS
+ * stream -- whatever the frame's place in the batch, the batch size or the variant called.  x_indent_cells and the
+ * block flags are ignored (the cursor move is the caller's prefix, as for the uniform sixel batch);
+ * B200TIMG_FAST_SCALE is accepted and ignored.  The default kernels always run (B200TIMG_EMIT, B200TIMG_DITHER_V1 and
+ * B200TIMG_PARTS do not apply).  Rejected with B200TIMG_EINVAL besides the cases above: out_w > 4095 and a padded
+ * height over 65536 rows (the message names the frame; wider images go through the uniform batch).
+ * The _dev variant follows the OUTPUT CAPACITY CONTRACT above.  The host variant stages into the sum of
+ * b200timg_sixel_bound(out_w, round_to_sixel(out_h)) over the frames and returns B200TIMG_ENOSPC with offsets[]
+ * complete and nothing written at or beyond out_cap.  b200timg_sixel_debug then reports frame 0. */
+int b200timg_sixel_mixed_dev(b200timg_ctx *ctx, const b200timg_mixed_batch *b, const uint8_t *d_src,
+                             char *d_out, size_t out_cap, uint64_t *d_offsets);
+int b200timg_sixel_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *b, const uint8_t *src,
+                         char *out, size_t out_cap, uint64_t *offsets);
 
 /* Device-resident single stages, for tests and for callers that keep frames on the GPU
  * (e.g. an NVDEC front end).  All pointers are DEVICE pointers. */

@@ -101,6 +101,8 @@ ABI = {
     "b200timg_scale_mixed_dev": (C.c_int, [C.c_void_p, C.POINTER(MixedBatch), C.c_void_p, C.c_void_p]),
     "b200timg_blocks_mixed_dev": (C.c_int, [C.c_void_p, C.POINTER(MixedBatch), C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200timg_blocks_mixed": (C.c_int, [C.c_void_p, C.POINTER(MixedBatch), C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200timg_sixel_mixed_dev": (C.c_int, [C.c_void_p, C.POINTER(MixedBatch), C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200timg_sixel_mixed": (C.c_int, [C.c_void_p, C.POINTER(MixedBatch), C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200timg_scale_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                      C.c_int, C.c_int]),
     "b200timg_compose_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint32,
@@ -495,6 +497,40 @@ class Context:
             d_offsets = torch.empty(n + 1, dtype=torch.int64, device=d_src.device)
         self._chk(lib().b200timg_blocks_mixed_dev(self.h, C.byref(b), d_src.data_ptr(), d_out.data_ptr(), out_cap,
                                                   d_offsets.data_ptr()))
+        return d_out, d_offsets
+
+    @staticmethod
+    def sixel_mixed_bound(outs):
+        """Staging bytes of a sixel mixed batch: the sum of b200timg_sixel_bound(out_w, round_to_sixel(out_h))."""
+        return sum(lib().b200timg_sixel_bound(ow, (oh + 5) // 6 * 6) for ow, oh in outs)
+
+    def sixel_mixed(self, images, outs, src_fmt=FMT_RGBA, has_bg=True, bg=0xFF000000, pattern=0, pattern_w=0, pattern_h=0):
+        """b200timg_sixel_mixed (host buffers): each frame's sixel stream, as a list of bytes."""
+        flat, offs = pack_mixed(images)
+        b, keep = mixed_batch([im.shape for im in images], outs, offs, None, 0, src_fmt, has_bg, bg, pattern, pattern_w,
+                              pattern_h)
+        n = len(outs)
+        cap = self.sixel_mixed_bound(outs)
+        out = np.empty(cap, np.uint8)
+        o = np.zeros(n + 1, np.uint64)
+        self._chk(lib().b200timg_sixel_mixed(self.h, C.byref(b), flat.ctypes.data, out.ctypes.data, cap, o.ctypes.data))
+        return [out[int(o[i]):int(o[i + 1])].tobytes() for i in range(n)]
+
+    def sixel_mixed_dev(self, d_src, b, d_out=None, out_cap=None, d_offsets=None):
+        """b200timg_sixel_mixed_dev on a packed source tensor (see pack_mixed / mixed_batch): returns (d_out, d_offsets)
+        after the (asynchronous) call -- device_sync() before reading them; d_out defaults to the sum of the frames' sixel
+        bounds."""
+        import torch
+        n = b.n_frames
+        if d_out is None:
+            cap = self.sixel_mixed_bound([(b.frames[f].out_w, b.frames[f].out_h) for f in range(n)])
+            d_out = torch.empty(cap, dtype=torch.uint8, device=d_src.device)
+        if out_cap is None:
+            out_cap = d_out.numel()
+        if d_offsets is None:
+            d_offsets = torch.empty(n + 1, dtype=torch.int64, device=d_src.device)
+        self._chk(lib().b200timg_sixel_mixed_dev(self.h, C.byref(b), d_src.data_ptr(), d_out.data_ptr(), out_cap,
+                                                 d_offsets.data_ptr()))
         return d_out, d_offsets
 
     def graphics_batch_dev(self, d_src, b, protocol, rgb24=False, ids=None, d_out=None, out_cap=None, d_offsets=None,

@@ -810,6 +810,70 @@ int b200timg_blocks_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *b, cons
     return sync(ctx);
 }
 
+// What the sixel encoder cannot take beyond validate_mixed: emit5's entry word holds x in 12 bits (wider frames take the
+// look-back emitter of the uniform batch), and the ditherer's per-band progress table holds 2048 bands of 32 rows.
+static int validate_sixel_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *b) {
+    B2_TRY(validate_mixed(ctx, b, false));
+    for (int f = 0; f < b->n_frames; ++f) {
+        const b200timg_frame &F = b->frames[f];
+        if (F.out_w > 4095)
+            return ctx->fail(B200TIMG_EINVAL, "sixel mixed batch: frame %d: width %d, at most 4095 (use the uniform batch)", f, F.out_w);
+        if ((round_to_sixel(F.out_h) + 31) / 32 > 2048)
+            return ctx->fail(B200TIMG_EINVAL, "sixel mixed batch: frame %d: height %d, the sixel path takes at most 65536 rows", f, F.out_h);
+    }
+    return B200TIMG_OK;
+}
+
+int b200timg_sixel_mixed_dev(b200timg_ctx *ctx, const b200timg_mixed_batch *b, const uint8_t *d_src,
+                             char *d_out, size_t out_cap, uint64_t *d_offsets) {
+    B2_TRY(check_ctx(ctx));
+    B2_TRY(validate_sixel_mixed(ctx, b));
+    if (!d_src || !d_out || !d_offsets) return ctx->fail(B200TIMG_EINVAL, "mixed batch: null pointer");
+    if (reinterpret_cast<uintptr_t>(d_src) & 3) return ctx->fail(B200TIMG_EINVAL, "mixed batch: pixel buffers must be 4-byte aligned");
+    MixedPlan mp;
+    B2_TRY(plan_scale_mixed(ctx, b, mp, true));
+    B2_TRY(plan_sixel_mixed(ctx, b, mp));
+    ctx->resident_fb = nullptr;
+    B2_CUDA(ctx, ctx->fb_scaled.reserve((size_t)mp.out_px * 4));
+    B2_TRY(mixed_upload(ctx, mp));
+    const ComposeSpec cs = make_compose_spec(b->has_bg, b->bg, b->pattern, b->pattern_w, b->pattern_h);
+    uint8_t *d_fb = ctx->fb_scaled.as<uint8_t>();
+    const char *d_arena = ctx->mixed_arena.as<char>();
+    B2_TRY(launch_scale_mixed(ctx, mp, d_arena, d_src, d_fb, b->n_frames, b->src_fmt == B200TIMG_FMT_RGB32, cs));
+    B2_TRY(launch_pad_mixed(ctx, mp, d_arena, d_fb, b->n_frames, cs));
+    return launch_sixel_mixed(ctx, mp, d_arena, d_fb, b->n_frames, d_out, out_cap, d_offsets);
+}
+
+// As b200timg_blocks_mixed: staging bounded by the sum of the frames' sixel bounds, offsets read back, then exactly the
+// encoded bytes (or nothing, with ENOSPC).
+int b200timg_sixel_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *b, const uint8_t *src,
+                         char *out, size_t out_cap, uint64_t *offsets) {
+    B2_TRY(check_ctx(ctx));
+    B2_TRY(validate_sixel_mixed(ctx, b));
+    if (!src || !out || !offsets) return ctx->fail(B200TIMG_EINVAL, "mixed batch: null pointer");
+    const int n = b->n_frames;
+    size_t src_bytes = 0, bound = 0;
+    for (int f = 0; f < n; ++f) {
+        const b200timg_frame &F = b->frames[f];
+        src_bytes = std::max(src_bytes, (size_t)F.src_offset + (size_t)F.src_w * F.src_h * 4);
+        bound += b200timg_sixel_bound(F.out_w, round_to_sixel(F.out_h));
+    }
+    B2_CUDA(ctx, ctx->in_stage.reserve(src_bytes));
+    B2_CUDA(ctx, ctx->out_stage.reserve(bound));
+    B2_CUDA(ctx, ctx->offsets.reserve((size_t)(n + 1) * sizeof(uint64_t)));
+    B2_CUDA(ctx, ctx->pinned.reserve((size_t)(n + 1) * sizeof(uint64_t)));
+    B2_TRY(upload(ctx, ctx->in_stage.p, src, src_bytes));
+    B2_TRY(b200timg_sixel_mixed_dev(ctx, b, ctx->in_stage.as<uint8_t>(), ctx->out_stage.as<char>(), bound, ctx->offsets.as<uint64_t>()));
+    B2_TRY(download(ctx, ctx->pinned.p, ctx->offsets.p, (size_t)(n + 1) * sizeof(uint64_t)));
+    B2_TRY(sync(ctx));
+    memcpy(offsets, ctx->pinned.p, (size_t)(n + 1) * sizeof(uint64_t));
+    const size_t total = (size_t)offsets[n];
+    if (total > bound) return ctx->fail(B200TIMG_ECUDA, "sixel mixed batch: encoded size %zu exceeds the bound %zu", total, bound);
+    if (total > out_cap) return ctx->fail(B200TIMG_ENOSPC, "sixel mixed batch: need %zu bytes (have %zu)", total, out_cap);
+    if (total) B2_TRY(download(ctx, out, ctx->out_stage.p, total));
+    return sync(ctx);
+}
+
 int b200timg_blocks_batch(b200timg_ctx *ctx, const b200timg_batch *b, const uint8_t *src, char *out,
                           size_t out_cap, uint64_t *offsets) {
     return batch_host(ctx, b, src, out, out_cap, offsets, Encoder::blocks);

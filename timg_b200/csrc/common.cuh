@@ -292,6 +292,12 @@ struct MixedPlan {
     unsigned long long out_px = 0;                 // scaled pixels of the whole batch
     unsigned rowpairs = 0;                         // block encoder: (frame, row pair) items ...
     unsigned long long cells = 0;                  // ... and cell records
+    // sixel encoder (plan_sixel_mixed): arena offsets of its descriptors and item lists, the sizes of its workspace parts
+    size_t o_sixel = 0, o_sband = 0, o_scta = 0, o_slist[2] = {0, 0};
+    int sixel_list[2] = {0, 0};                    // frames whose median-cut tables fit shared memory / need global memory
+    unsigned sixel_bands = 0, sixel_ctas = 0;      // flat (frame, band) and (frame, dither CTA) items
+    int sixel_nwarps = 0, sixel_wmax = 0, sixel_split = 0;
+    size_t sixel_pal_smem = 0, sixel_ent = 0, sixel_idx = 0, sixel_bnd = 0, sixel_scr = 0, sixel_prog = 0;
 };
 // appends bytes at a 16-byte boundary of the arena and returns their offset
 inline size_t mixed_put(std::vector<char> &a, const void *p, size_t bytes) {
@@ -300,12 +306,21 @@ inline size_t mixed_put(std::vector<char> &a, const void *p, size_t bytes) {
     if (bytes) memcpy(a.data() + o, p, bytes);
     return o;
 }
-int plan_scale_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *b, MixedPlan &mp);
+// sixel_rows: every frame's output takes round_to_sixel(out_h) rows (the sixel encoder's padded frames)
+int plan_scale_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *b, MixedPlan &mp, bool sixel_rows = false);
 int plan_blocks_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *b, MixedPlan &mp);
 // scale + fused compose of every frame into d_out (frames back to back)
 int launch_scale_mixed(b200timg_ctx *ctx, const MixedPlan &mp, const char *d_arena, const uint8_t *d_src, uint8_t *d_out,
                        int n_frames, int bgra, const ComposeSpec &cs);
 int launch_blocks_mixed(b200timg_ctx *ctx, const MixedPlan &mp, const char *d_arena, const uint8_t *d_fb, int n_frames,
                         int flags, char *d_out, size_t out_cap, uint64_t *d_offsets);
+// the sixel encoder's pad strips (rows out_h .. round_to_sixel(out_h) - 1: transparent, then composed) of a plan made
+// with sixel_rows
+int launch_pad_mixed(b200timg_ctx *ctx, const MixedPlan &mp, const char *d_arena, uint8_t *d_out, int n_frames, const ComposeSpec &cs);
+// palette -> table -> map / dither -> emit5 -> layout -> offsets -> compaction of the padded frames of a plan made with
+// sixel_rows; plan_sixel_mixed adds the encoder's descriptors to the arena and reserves ctx->sixel_work
+int plan_sixel_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *b, MixedPlan &mp);
+int launch_sixel_mixed(b200timg_ctx *ctx, const MixedPlan &mp, const char *d_arena, const uint8_t *d_fb, int n_frames,
+                       char *d_out, size_t out_cap, uint64_t *d_offsets);
 
 }  // namespace b200timg

@@ -1710,6 +1710,7 @@ struct __align__(16) MixedScaleFrame {
     unsigned long long tab;        // this geometry's tables, in 4-byte words from the table arena:
                                    // h_first[ow] h_count[ow] v_first[oh] v_count[oh] h_coeff[ow][hw] v_coeff[oh][vw]
     int iw, ih, ow, oh, h_widest, v_widest, vertical_first, h_sequential, copy_only;
+    int out_rows;                  // rows the frame takes in the output: oh, or the sixel encoder's multiple of 6
 };
 
 // frame that owns flat item b: the last f with start[f] <= b (frames without items share their start)
@@ -1835,7 +1836,7 @@ mixed_pass2_kernel(MixedScaleArgs A) {
 
 // Tables and descriptors of every frame; frames of equal geometry share one plan.  Frame groups bound the float
 // intermediate: a group closes before the frame that would take it past the budget (a frame alone may exceed it).
-int plan_scale_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *mb, MixedPlan &mp) {
+int plan_scale_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *mb, MixedPlan &mp, bool sixel_rows) {
     const int n = mb->n_frames;
     unsigned long long budget = 2ull << 30;
     if (const char *e = getenv("B200TIMG_MIXED_GROUP_BYTES")) budget = std::max(1ull, strtoull(e, nullptr, 10));   // test knob
@@ -1873,6 +1874,7 @@ int plan_scale_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *mb, MixedPla
         D.iw = F.src_w; D.ih = F.src_h; D.ow = F.out_w; D.oh = F.out_h;
         D.h_widest = G.hw; D.v_widest = G.vw;
         D.vertical_first = G.vertical_first; D.h_sequential = G.h_sequential; D.copy_only = G.copy_only;
+        D.out_rows = sixel_rows ? (F.out_h + 5) / 6 * 6 : F.out_h;
         const unsigned long long elems = D.copy_only ? 0ull
                                        : D.vertical_first ? (unsigned long long)F.out_h * F.src_w : (unsigned long long)F.src_h * F.out_w;
         if (group_tmp && (group_tmp + elems) * sizeof(float4) > budget) { mp.group_end.push_back(f); group_tmp = 0; }
@@ -1882,7 +1884,7 @@ int plan_scale_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *mb, MixedPla
         mp.p1[f] = (unsigned)p1; mp.p2[f] = (unsigned)p2;
         p1 += (elems + 255) / 256;
         p2 += ((unsigned long long)F.out_w * F.out_h + 255) / 256;
-        out_px += (unsigned long long)F.out_w * F.out_h;
+        out_px += (unsigned long long)F.out_w * D.out_rows;
         if (p1 > 0x7fffffffull || p2 > 0x7fffffffull)
             return ctx->fail(B200TIMG_EINVAL, "mixed batch: more than 2^31 - 1 scaler work items in one call (at frame %d)", f);
     }
@@ -1893,6 +1895,27 @@ int plan_scale_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *mb, MixedPla
     mp.o_p1 = mixed_put(mp.arena, mp.p1.data(), sizeof(unsigned) * (n + 1));
     mp.o_p2 = mixed_put(mp.arena, mp.p2.data(), sizeof(unsigned) * (n + 1));
     mp.o_tab = mixed_put(mp.arena, tab.data(), sizeof(int32_t) * tab.size());
+    return B200TIMG_OK;
+}
+
+// The sixel encoder's pad strip of every frame (rows oh .. out_rows - 1), one CTA per frame: what the uniform batch does
+// with a memset and a compose from start_row = oh (SixelCanvas::Send, src/sixel-canvas.cc:109-120).
+__global__ void __launch_bounds__(256)
+mixed_pad_kernel(const MixedScaleFrame *__restrict__ frames, uint32_t *__restrict__ out, ComposeSpec cs) {
+    const MixedScaleFrame F = frames[blockIdx.x];
+    const int n = (F.out_rows - F.oh) * F.ow;
+    uint32_t *strip = out + F.out_px + (long long)F.oh * F.ow;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const int y = i / F.ow, x = i - y * F.ow;
+        strip[i] = compose_at(cs, 0u, x, F.oh + y);
+    }
+}
+
+int launch_pad_mixed(b200timg_ctx *ctx, const MixedPlan &mp, const char *d_arena, uint8_t *d_out, int n_frames, const ComposeSpec &cs) {
+    B2_KERNEL(ctx, "mixed_pad_kernel");
+    mixed_pad_kernel<<<n_frames, 256, 0, ctx->stream>>>(reinterpret_cast<const MixedScaleFrame *>(d_arena + mp.o_scale),
+                                                        reinterpret_cast<uint32_t *>(d_out), cs);
+    B2_LAUNCH_CHECK(ctx);
     return B200TIMG_OK;
 }
 

@@ -44,11 +44,43 @@ __device__ __forceinline__ int pick_plane(int d0, int d1, int d2) {
     return plane;
 }
 
+// ---- per-frame geometry of the front and back kernels ------------------------------------------------------------
+// Each kernel below reads the quantities that differ between frames through an accessor:
+//   *Uniform  a b200timg_batch: every frame has the launch's geometry, frame f at f times the frame size, the CTA's frame
+//             and item from blockIdx as before (these instantiations compile to the same SASS as the plain kernels did)
+//   *Mixed    a mixed batch: a MixedSixelFrame per frame and flat item lists (MixedSixelParams)
+struct NoMixed {};                        // the uniform kernels' (unused) last parameter
+
+struct PaletteUniform {                   // one CTA per frame
+    typedef NoMixed Params;
+    int w, h; const SixelWork &W; int f;
+    __device__ __forceinline__ PaletteUniform(int w_, int h_, const SixelWork &W_, const NoMixed &) : w(w_), h(h_), W(W_), f(blockIdx.x) {}
+    __device__ __forceinline__ bool skip() const { return false; }
+    __device__ __forceinline__ long long npix() const { return (long long)w * h; }
+    __device__ __forceinline__ long long px0(long long n) const { return (long long)f * n; }
+    __device__ __forceinline__ int ent_cap() const { return W.ent_cap; }
+    __device__ __forceinline__ long long ent0() const { return (long long)f * W.ent_cap; }
+};
+struct PaletteMixed {                     // one CTA per listed frame (a launch may list none: one idle CTA)
+    typedef MixedSixelParams Params;
+    MixedSixelFrame D; int f; bool out;
+    __device__ __forceinline__ PaletteMixed(int, int, const SixelWork &, const MixedSixelParams &P) {
+        out = (int)blockIdx.x >= P.n_list;
+        f = out ? 0 : P.list[blockIdx.x];
+        D = P.desc[f];
+    }
+    __device__ __forceinline__ bool skip() const { return out; }
+    __device__ __forceinline__ long long npix() const { return (long long)D.w * D.h; }
+    __device__ __forceinline__ long long px0(long long) const { return (long long)D.fb_px; }
+    __device__ __forceinline__ int ent_cap() const { return D.ent_cap; }
+    __device__ __forceinline__ long long ent0() const { return (long long)D.ent; }
+};
+
 // SMEM_TABLES: the two median-cut tables live in shared memory (the histogram aliases the second
 // one: it is dead once the first is compacted); otherwise they are in global memory (L2).
-template <bool SMEM_TABLES>
+template <bool SMEM_TABLES, class G>
 __global__ void __launch_bounds__(PT)
-sixel_palette_kernel(const uint32_t *__restrict__ fb, int w, int h, SixelWork W) {
+sixel_palette_kernel(const uint32_t *__restrict__ fb, int w, int h, SixelWork W, typename G::Params M) {
     extern __shared__ uint32_t s_hist[];               // 16384 words: two u16 counters per word (then table T)
     __shared__ uint32_t s_w[PT / 32];
     __shared__ int b_ind[256], b_col[256], b_med[256], t_ind[256], t_col[256], t_med[256];   // b_med: cached split (-1: none)
@@ -60,13 +92,15 @@ sixel_palette_kernel(const uint32_t *__restrict__ fb, int w, int h, SixelWork W)
     __shared__ int s_todo[32], s_ntodo, s_boxes, s_done;
     __shared__ unsigned long long s_med;
 
-    const int f = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    const long long npix = (long long)w * h;
-    const uint32_t *frame = fb + (long long)f * npix;
+    const G g(w, h, W, M);
+    if (g.skip()) return;
+    const int f = g.f, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const long long npix = g.npix();
+    const uint32_t *frame = fb + g.px0(npix);
     SixelFrameHdr *hdr = W.hdr + f;
-    const int t_words = W.ent_cap > 16384 ? W.ent_cap : 16384;
-    uint32_t *E = SMEM_TABLES ? s_hist + t_words : W.ent_a + (long long)f * W.ent_cap;
-    uint32_t *T = SMEM_TABLES ? s_hist : W.ent_b + (long long)f * W.ent_cap;
+    const int t_words = g.ent_cap() > 16384 ? g.ent_cap() : 16384;
+    uint32_t *E = SMEM_TABLES ? s_hist + t_words : W.ent_a + g.ent0();
+    uint32_t *T = SMEM_TABLES ? s_hist : W.ent_b + g.ent0();
 
     // quant.c computeHistogram, QUALITY_LOW: step = length/depth/max_sample*depth (bytes)
     unsigned long long step_px = (unsigned long long)npix / 18383ull;
@@ -390,15 +424,34 @@ sixel_lut_kernel(SixelWork W) {
     W.lut[(long long)f * 32768 + cell] = (uint8_t)bi;
 }
 
+struct MapUniform {                       // frame blockIdx.y
+    typedef NoMixed Params;
+    long long n; int f;
+    __device__ __forceinline__ MapUniform(long long npix, const NoMixed &, int f_) : n(npix), f(f_) {}
+    __device__ __forceinline__ long long npix() const { return n; }
+    __device__ __forceinline__ long long px0() const { return (long long)f * n; }
+    __device__ __forceinline__ long long idx0() const { return (long long)f * n; }
+};
+struct MapMixed {
+    typedef MixedSixelParams Params;
+    MixedSixelFrame D;
+    __device__ __forceinline__ MapMixed(long long, const MixedSixelParams &P, int f) : D(P.desc[f]) {}
+    __device__ __forceinline__ long long npix() const { return (long long)D.w * D.h; }
+    __device__ __forceinline__ long long px0() const { return (long long)D.fb_px; }
+    __device__ __forceinline__ long long idx0() const { return (long long)D.idx; }
+};
+
 // no diffusion (<= 256 distinct sampled colours): plain table lookup per pixel
+template <class G>
 __global__ void __launch_bounds__(256)
-sixel_map_kernel(const uint32_t *__restrict__ fb, long long npix, SixelWork W) {
+sixel_map_kernel(const uint32_t *__restrict__ fb, long long npix, SixelWork W, typename G::Params M) {
     const int f = blockIdx.y;
     if (W.hdr[f].diffuse) return;
     const uint8_t *lut = W.lut + (long long)f * 32768;
+    const G g(npix, M, f);
     const long long stride = (long long)gridDim.x * blockDim.x;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < npix; i += stride)
-        W.index[(long long)f * npix + i] = lut[hash15(fb[(long long)f * npix + i])];
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < g.npix(); i += stride)
+        W.index[g.idx0() + i] = lut[hash15(fb[g.px0() + i])];
 }
 
 // ---- Floyd-Steinberg wavefront --------------------------------------------------------------
@@ -793,17 +846,54 @@ __device__ unsigned long long g_emit_clocks[2][EMIT_CLK_PHASES];     // [0: emit
 //     32 sectors.
 constexpr int ROW_WORDS = (6 * 32 * STASH_STEPS * EW + 3) / 4 / ET + 1;   // words of the staged rows per thread (+1: misalignment)
 
-template <bool V5>
+// Band accessors (emit, compaction): the CTA's frame and 6-row band, where the band's index rows, size, offset and
+// scratch slot live.
+template <class Dims>                     // EmitGeom (emit) or NoMixed (compaction): the kernels' parameters as before
+struct BandUniform {                      // band blockIdx.x of frame blockIdx.y
+    typedef Dims Params;
+    const Dims &G; int band, f;
+    __device__ __forceinline__ explicit BandUniform(const Dims &g) : G(g), band(blockIdx.x), f(blockIdx.y) {}
+    __device__ __forceinline__ int w() const { return G.w; }
+    __device__ __forceinline__ int cols_per_warp() const { return G.cols_per_warp; }
+    __device__ __forceinline__ int width(int w_) const { return w_; }      // compaction: its own w / h parameters
+    __device__ __forceinline__ int height(int h_) const { return h_; }
+    __device__ __forceinline__ int nbands(const SixelWork &W) const { return W.nbands; }
+    __device__ __forceinline__ long long idx0(int w_) const { return ((long long)f * G.h + (long long)band * 6) * w_; }
+    __device__ __forceinline__ long long slot(const SixelWork &W) const { return (long long)f * W.nbands + band; }
+    __device__ __forceinline__ size_t scr(const SixelWork &W) const { return ((size_t)f * W.nbands + band) * W.band_cap; }
+};
+typedef BandUniform<EmitGeom> EmitBands;
+typedef BandUniform<NoMixed> CompactBands;
+struct BandMixed {                        // flat band blockIdx.x
+    typedef MixedSixelParams Params;
+    MixedSixelFrame D; int band, f;
+    __device__ __forceinline__ explicit BandMixed(const MixedSixelParams &P) {
+        f = sixel_owner(P.band_start, P.n_frames, blockIdx.x);
+        band = (int)(blockIdx.x - P.band_start[f]);
+        D = P.desc[f];
+    }
+    __device__ __forceinline__ int w() const { return D.w; }
+    __device__ __forceinline__ int cols_per_warp() const { return D.cols_per_warp; }
+    __device__ __forceinline__ int width(int) const { return D.w; }
+    __device__ __forceinline__ int height(int) const { return D.h; }
+    __device__ __forceinline__ int nbands(const SixelWork &) const { return D.nbands; }
+    __device__ __forceinline__ long long idx0(int w_) const { return (long long)D.idx + (long long)band * 6 * w_; }
+    __device__ __forceinline__ long long slot(const SixelWork &) const { return (long long)D.band0 + band; }
+    __device__ __forceinline__ size_t scr(const SixelWork &) const { return (size_t)D.scr + (size_t)band * D.band_cap; }
+};
+
+template <bool V5, class A>
 __global__ void __launch_bounds__(ET, 2)
-sixel_emit1b_kernel(EmitGeom G, SixelWork W) {
+sixel_emit1b_kernel(typename A::Params G, SixelWork W) {
     extern __shared__ uint32_t s_sorted[];                   // [6*w]
     __shared__ uint32_t s_tab[SLOT_WORDS * ET];              // sort: cnt[EW][256] | mask[EW][256]; afterwards: slots
     __shared__ uint32_t s_w[ET / 32];
-    const int band = blockIdx.x, f = blockIdx.y, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    const int w = G.w;
-    const uint8_t *idx = W.index + ((long long)f * G.h + (long long)band * 6) * w;
+    const A a(G);
+    const int band = a.band, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const int w = a.w();
+    const uint8_t *idx = W.index + a.idx0(w);
     EMIT_CLK_BEGIN;
-    const bool stash = G.cols_per_warp <= 32 * STASH_STEPS;
+    const bool stash = a.cols_per_warp() <= 32 * STASH_STEPS;
     const uint8_t *cols = idx;                               // where the count pass reads the band's rows
     if (V5 && stash) {
         // aligned words covering [idx, idx + 6w).  The <= 3 bytes outside the band stay inside the index region: sixel_plan
@@ -826,7 +916,7 @@ sixel_emit1b_kernel(EmitGeom G, SixelWork W) {
     if (!V5) EMIT_CLK();                                     // zero
     // (1) the sort: as in v1, but the column entries (<= 6 distinct colours of a column with their row bits) are computed
     // once: the count pass parks them in registers (3 words per 32-column step, steps unrolled) for the scatter pass
-    const int x_lo = wid * G.cols_per_warp, x_hi = min(w, x_lo + G.cols_per_warp);
+    const int x_lo = wid * a.cols_per_warp(), x_hi = min(w, x_lo + a.cols_per_warp());
     uint32_t *cnt = s_tab + wid * 256, *M = s_tab + EW * 256 + wid * 256;
     uint32_t k0[STASH_STEPS], k1[STASH_STEPS], k2[STASH_STEPS];     // colours 0-3 | colours 4-5, valid, bits 5 | bits 0-4
     if (stash) {
@@ -931,11 +1021,11 @@ sixel_emit1b_kernel(EmitGeom G, SixelWork W) {
     const uint32_t local = pos;
     EMIT_CLK();                                              // walk
     uint32_t band_total; const uint32_t at = block_excl_scan<ET>(local, s_w, band_total);
-    if (tid == 0) W.band_bytes[(long long)f * W.nbands + band] = band_total;
+    if (tid == 0) W.band_bytes[a.slot(W)] = band_total;
     EMIT_CLK();                                              // scan
     // (3) the slot's bytes to `at` of this band's 16-byte aligned scratch place (v1b), or of its image in shared memory
     // (emit5): head bytes up to a word boundary, whole words realigned with a funnel shift, tail bytes
-    char *const band_out = W.scratch + ((size_t)f * W.nbands + band) * W.band_cap;
+    char *const band_out = W.scratch + a.scr(W);
     char *o = band_out + at;
     auto slot_out = [&](char *d) {
         const uint32_t head = min(local, (4u - (at & 3u)) & 3u);
@@ -978,11 +1068,32 @@ sixel_emit1b_kernel(EmitGeom G, SixelWork W) {
 }
 
 // per frame: header length, band offsets (exclusive, in place), frame size
+struct LayoutUniform {                    // frame blockIdx.x
+    typedef NoMixed Params;
+    const SixelWork &W; int f;
+    __device__ __forceinline__ LayoutUniform(const SixelWork &W_, const NoMixed &, int f_) : W(W_), f(f_) {}
+    __device__ __forceinline__ int w(int w_) const { return w_; }
+    __device__ __forceinline__ int h(int h_) const { return h_; }
+    __device__ __forceinline__ int nbands() const { return W.nbands; }
+    __device__ __forceinline__ long long band0() const { return (long long)f * W.nbands; }
+};
+struct LayoutMixed {
+    typedef MixedSixelParams Params;
+    MixedSixelFrame D;
+    __device__ __forceinline__ LayoutMixed(const SixelWork &, const MixedSixelParams &P, int f) : D(P.desc[f]) {}
+    __device__ __forceinline__ int w(int) const { return D.w; }
+    __device__ __forceinline__ int h(int) const { return D.h; }
+    __device__ __forceinline__ int nbands() const { return D.nbands; }
+    __device__ __forceinline__ long long band0() const { return (long long)D.band0; }
+};
+
+template <class G>
 __global__ void __launch_bounds__(256)
-sixel_layout_kernel(int w, int h, SixelWork W) {
+sixel_layout_kernel(int w, int h, SixelWork W, typename G::Params M) {
     __shared__ uint32_t s_w[8];
     __shared__ uint32_t s_carry;
     const int f = blockIdx.x, tid = threadIdx.x;
+    const G lay(W, M, f);
     SixelFrameHdr *hdr = W.hdr + f;
     uint32_t len = 0;
     if ((uint32_t)tid < hdr->ncolors) {
@@ -991,15 +1102,15 @@ sixel_layout_kernel(int w, int h, SixelWork W) {
         len = 1 + ndig_u((uint32_t)tid) + 3 + ndig_u(r) + 1 + ndig_u(g) + 1 + ndig_u(b);
     }
     uint32_t pal_total; (void)block_excl_scan<256>(len, s_w, pal_total);
-    const uint32_t header = 8 + ndig_u((uint32_t)w) + 1 + ndig_u((uint32_t)h) + pal_total;
+    const uint32_t header = 8 + ndig_u((uint32_t)lay.w(w)) + 1 + ndig_u((uint32_t)lay.h(h)) + pal_total;
     if (tid == 0) s_carry = header;
     __syncthreads();
-    uint32_t *bb = W.band_bytes + (long long)f * W.nbands;
-    for (int b0 = 0; b0 < W.nbands; b0 += 256) {
+    uint32_t *bb = W.band_bytes + lay.band0();
+    for (int b0 = 0; b0 < lay.nbands(); b0 += 256) {
         const int b = b0 + tid;
-        const uint32_t v = b < W.nbands ? bb[b] + (b > 0 ? 1u : 0u) : 0;       // '-' before every band but the first
+        const uint32_t v = b < lay.nbands() ? bb[b] + (b > 0 ? 1u : 0u) : 0;       // '-' before every band but the first
         uint32_t tot; const uint32_t at = block_excl_scan<256>(v, s_w, tot);
-        if (b < W.nbands) W.band_off[(long long)f * W.nbands + b] = s_carry + at + (b > 0 ? 1u : 0u);   // band's first data byte
+        if (b < lay.nbands()) W.band_off[lay.band0() + b] = s_carry + at + (b > 0 ? 1u : 0u);   // band's first data byte
         __syncthreads();
         if (tid == 0) s_carry += tot;
         __syncthreads();
@@ -1034,17 +1145,19 @@ sixel_sizes_to_offsets_kernel(const SixelFrameHdr *__restrict__ hdr, int n, uint
 
 // Final assembly: header + palette (band 0's CTA), every band's bytes copied from its scratch slot
 // to its place in the compacted stream, '-' between bands, ST at the end.  Pure byte traffic.
+template <class A>
 __global__ void __launch_bounds__(256)
 sixel_compact_kernel(int w, int h, SixelWork W, const uint64_t *__restrict__ offsets, char *__restrict__ out,
-                     unsigned long long out_cap) {
+                     unsigned long long out_cap, typename A::Params M) {
     __shared__ uint32_t s_w[8];
-    const int band = blockIdx.x, f = blockIdx.y, tid = threadIdx.x;
+    const A a(M);
+    const int band = a.band, f = a.f, tid = threadIdx.x;
     const SixelFrameHdr *hdr = W.hdr + f;
     const unsigned long long fbase = offsets[f];
     if (fbase + hdr->frame_size > out_cap) return;           // never write out of bounds
-    const uint32_t boff = W.band_off[(long long)f * W.nbands + band];
-    const uint32_t n = W.band_bytes[(long long)f * W.nbands + band];
-    const char *src = W.scratch + ((size_t)f * W.nbands + band) * W.band_cap;
+    const uint32_t boff = W.band_off[a.slot(W)];
+    const uint32_t n = W.band_bytes[a.slot(W)];
+    const char *src = W.scratch + a.scr(W);
     char *dst = out + fbase + boff;
     {   // word copy: 4-byte aligned stores, source words realigned with a funnel shift
         const uint32_t head = min(n, (uint32_t)((4 - (reinterpret_cast<uintptr_t>(dst) & 3)) & 3));
@@ -1058,15 +1171,15 @@ sixel_compact_kernel(int w, int h, SixelWork W, const uint64_t *__restrict__ off
     }
     if (tid == 0) {
         if (band > 0) dst[-1] = '-';                         // DECGNL between bands
-        if (band == W.nbands - 1) { out[fbase + hdr->frame_size - 2] = '\033'; out[fbase + hdr->frame_size - 1] = '\\'; }
+        if (band == a.nbands(W) - 1) { out[fbase + hdr->frame_size - 2] = '\033'; out[fbase + hdr->frame_size - 1] = '\\'; }
     }
     if (band == 0) {                                         // DCS q, raster attributes, palette definitions
         if (tid == 0) {
             char *o = out + fbase;
             *o++ = '\033'; *o++ = 'P'; *o++ = 'q'; *o++ = '"'; *o++ = '1'; *o++ = ';'; *o++ = '1'; *o++ = ';';
-            o = put_num_u(o, (uint32_t)w); *o++ = ';'; o = put_num_u(o, (uint32_t)h);
+            o = put_num_u(o, (uint32_t)a.width(w)); *o++ = ';'; o = put_num_u(o, (uint32_t)a.height(h));
         }
-        const uint32_t fixed = 8 + ndig_u((uint32_t)w) + 1 + ndig_u((uint32_t)h);
+        const uint32_t fixed = 8 + ndig_u((uint32_t)a.width(w)) + 1 + ndig_u((uint32_t)a.height(h));
         uint32_t len = 0, r = 0, g = 0, b = 0;
         if ((uint32_t)tid < hdr->ncolors) {                  // output_rgb_palette_definition: (v*100+127)/255 percent
             const uint32_t p = hdr->palette[tid];
@@ -1159,13 +1272,13 @@ static int sixel_plan(b200timg_ctx *ctx, int w, int h, int n_frames, bool reserv
     const size_t smem_limit = 227 * 1024 - 36 * 1024;   // the emit kernel also has ~33 KB of static shared memory
     S->emit_smem = sizeof(uint32_t) * (size_t)6 * w;
     if (!ctx->sixel_attrs_set) {                         // function attributes are per device, i.e. per context
-        B2_CUDA(ctx, cudaFuncSetAttribute(sixel_palette_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 65536));
+        B2_CUDA(ctx, cudaFuncSetAttribute(sixel_palette_kernel<false, PaletteUniform>, cudaFuncAttributeMaxDynamicSharedMemorySize, 65536));
         B2_CUDA(ctx, cudaFuncSetAttribute(sixel_emit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit));
-        B2_CUDA(ctx, cudaFuncSetAttribute(sixel_emit1b_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (227 - 47) * 1024));
-        B2_CUDA(ctx, cudaFuncSetAttribute(sixel_emit1b_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (227 - 47) * 1024));
+        B2_CUDA(ctx, cudaFuncSetAttribute(sixel_emit1b_kernel<false, EmitBands>, cudaFuncAttributeMaxDynamicSharedMemorySize, (227 - 47) * 1024));
+        B2_CUDA(ctx, cudaFuncSetAttribute(sixel_emit1b_kernel<true, EmitBands>, cudaFuncAttributeMaxDynamicSharedMemorySize, (227 - 47) * 1024));
         B2_CUDA(ctx, cudaFuncSetAttribute(sixel_dither_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 32768 + DW_MAX * DWARP_SMEM));
         // unconditionally: which variant a frame takes depends on ITS size, not on the first frame this context saw
-        B2_CUDA(ctx, cudaFuncSetAttribute(sixel_palette_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        B2_CUDA(ctx, cudaFuncSetAttribute(sixel_palette_kernel<true, PaletteUniform>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
         ctx->sixel_attrs_set = true;
     }
     return B200TIMG_OK;
@@ -1188,8 +1301,8 @@ int launch_sixel_front(b200timg_ctx *ctx, const uint8_t *d_fb, int w, int h, int
     {
         const size_t t_words = W.ent_cap > 16384 ? (size_t)W.ent_cap : 16384;
         const size_t smem_tables = sizeof(uint32_t) * (t_words + (size_t)W.ent_cap);
-        if (smem_tables <= 200 * 1024) sixel_palette_kernel<true><<<n, PT, smem_tables, ctx->stream>>>(fb, w, h, W);
-        else sixel_palette_kernel<false><<<n, PT, 65536, ctx->stream>>>(fb, w, h, W);
+        if (smem_tables <= 200 * 1024) sixel_palette_kernel<true, PaletteUniform><<<n, PT, smem_tables, ctx->stream>>>(fb, w, h, W, NoMixed());
+        else sixel_palette_kernel<false, PaletteUniform><<<n, PT, 65536, ctx->stream>>>(fb, w, h, W, NoMixed());
     }
     B2_LAUNCH_CHECK(ctx);
     B2_KERNEL(ctx, "sixel_lut_kernel");
@@ -1198,7 +1311,7 @@ int launch_sixel_front(b200timg_ctx *ctx, const uint8_t *d_fb, int w, int h, int
     {
         long long blocks = (npix + 255) / 256; if (blocks > 64) blocks = 64;
         B2_KERNEL(ctx, "sixel_map_kernel");
-        sixel_map_kernel<<<dim3((unsigned)blocks, n), 256, 0, ctx->stream>>>(fb, npix, W);
+        sixel_map_kernel<MapUniform><<<dim3((unsigned)blocks, n), 256, 0, ctx->stream>>>(fb, npix, W, NoMixed());
         B2_LAUNCH_CHECK(ctx);
     }
     if (!S.dither_v1) {
@@ -1215,8 +1328,8 @@ int launch_sixel_front(b200timg_ctx *ctx, const uint8_t *d_fb, int w, int h, int
     }
     if (S.emit_v1) {
         B2_KERNEL(ctx, S.emit_mode == 5 ? "sixel_emit5_kernel" : "sixel_emit_kernel");
-        if (S.emit_mode == 5) sixel_emit1b_kernel<true><<<dim3(W.nbands, n), ET, S.emit_smem, ctx->stream>>>(S.G, W);
-        else if (S.emit_mode == 4) sixel_emit1b_kernel<false><<<dim3(W.nbands, n), ET, S.emit_smem, ctx->stream>>>(S.G, W);
+        if (S.emit_mode == 5) sixel_emit1b_kernel<true, EmitBands><<<dim3(W.nbands, n), ET, S.emit_smem, ctx->stream>>>(S.G, W);
+        else if (S.emit_mode == 4) sixel_emit1b_kernel<false, EmitBands><<<dim3(W.nbands, n), ET, S.emit_smem, ctx->stream>>>(S.G, W);
         else sixel_emit_kernel<<<dim3(W.nbands, n), ET, S.emit_smem, ctx->stream>>>(S.G, W);
         B2_LAUNCH_CHECK(ctx);
     }
@@ -1235,7 +1348,7 @@ int launch_sixel_back(b200timg_ctx *ctx, int w, int h, int n_frames, char *d_out
     }
     if (phases & 1) {
         B2_KERNEL(ctx, "sixel_layout_kernel");
-        sixel_layout_kernel<<<n_frames, 256, 0, ctx->stream>>>(w, h, W);
+        sixel_layout_kernel<LayoutUniform><<<n_frames, 256, 0, ctx->stream>>>(w, h, W, NoMixed());
         B2_LAUNCH_CHECK(ctx);
         B2_KERNEL(ctx, "sixel_sizes_to_offsets_kernel");
         sixel_sizes_to_offsets_kernel<<<1, 1024, 0, ctx->stream>>>(W.hdr, n_frames, d_offsets);
@@ -1243,7 +1356,7 @@ int launch_sixel_back(b200timg_ctx *ctx, int w, int h, int n_frames, char *d_out
     }
     if (!(phases & 2)) return B200TIMG_OK;
     B2_KERNEL(ctx, "sixel_compact_kernel");
-    sixel_compact_kernel<<<dim3(W.nbands, n_frames), 256, 0, ctx->stream>>>(w, h, W, d_offsets, d_out, (unsigned long long)out_cap);
+    sixel_compact_kernel<CompactBands><<<dim3(W.nbands, n_frames), 256, 0, ctx->stream>>>(w, h, W, d_offsets, d_out, (unsigned long long)out_cap, NoMixed());
     B2_LAUNCH_CHECK(ctx);
     return B200TIMG_OK;
 }
@@ -1254,6 +1367,142 @@ int launch_sixel(b200timg_ctx *ctx, const uint8_t *d_fb, int w, int h, int n_fra
                  size_t out_cap, uint64_t *d_offsets, int phases) {
     if (phases & 1) B2_TRY(launch_sixel_front(ctx, d_fb, w, h, n_frames, 0, n_frames, true));
     return launch_sixel_back(ctx, w, h, n_frames, d_out, out_cap, d_offsets, phases);
+}
+
+// ---- mixed-geometry batches (b200timg_sixel_mixed_dev) -----------------------------------------------------------
+// The same kernels over frames of different geometry, in a fixed number of launches: the palette kernel twice (frames
+// whose median-cut tables fit shared memory, frames that need the global tables), then the table, map, dither, emit5,
+// layout, offsets and compaction kernels once each.  Each frame gets exactly what sixel_plan gives a one-frame batch of
+// its geometry (table size, band scratch, emit5's column split), so its bytes are that batch's.  Headers and tables stay
+// dense per frame; everything else is packed frame after frame and found through the frame's MixedSixelFrame.
+
+// ctx->sixel_work of a mixed plan: [hdr | ent_a | ent_b | lut | index | band sizes | band offsets | scratch | dither
+// boundary rows | dither progress]
+static size_t mixed_sixel_work(const MixedPlan &mp, int n, char *base, SixelWork *W, size_t *o_bnd, size_t *o_prog) {
+    size_t off = 0;
+    const size_t o_hdr = off; off += align_up(sizeof(SixelFrameHdr) * n, 256);
+    const size_t o_ea = off; off += align_up(sizeof(uint32_t) * mp.sixel_ent, 256);
+    const size_t o_eb = off; off += align_up(sizeof(uint32_t) * mp.sixel_ent, 256);
+    const size_t o_lut = off; off += align_up((size_t)32768 * n, 256);
+    const size_t o_idx = off; off += align_up(mp.sixel_idx, 256);
+    const size_t o_bb = off; off += align_up(sizeof(uint32_t) * mp.sixel_bands, 256);
+    const size_t o_bo = off; off += align_up(sizeof(uint32_t) * mp.sixel_bands, 256);
+    const size_t o_scr = off; off += align_up(mp.sixel_scr, 256);
+    *o_bnd = off; off += align_up(sizeof(uint4) * mp.sixel_bnd, 256);
+    *o_prog = off; off += align_up(sizeof(int) * mp.sixel_prog, 256);
+    if (W) {
+        *W = SixelWork{};
+        W->hdr = reinterpret_cast<SixelFrameHdr *>(base + o_hdr);
+        W->ent_a = reinterpret_cast<uint32_t *>(base + o_ea); W->ent_b = reinterpret_cast<uint32_t *>(base + o_eb);
+        W->lut = reinterpret_cast<uint8_t *>(base + o_lut); W->index = reinterpret_cast<uint8_t *>(base + o_idx);
+        W->band_bytes = reinterpret_cast<uint32_t *>(base + o_bb); W->band_off = reinterpret_cast<uint32_t *>(base + o_bo);
+        W->scratch = base + o_scr;
+    }
+    return off;
+}
+
+int plan_sixel_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *mb, MixedPlan &mp) {
+    const int n = mb->n_frames;
+    std::vector<MixedSixelFrame> desc(n);
+    std::vector<unsigned> band_start(n + 1), cta_start(n + 1);
+    std::vector<int> list[2];
+    unsigned long long px = 0;
+    size_t ent = 0, idx = 0, bnd = 0, scr = 0, prog = 0;
+    unsigned bands = 0, ctas = 0;
+    int nwarps = 1, wmax = 1, split = 0;
+    size_t pal_smem = 0;
+    for (int f = 0; f < n; ++f) {
+        const b200timg_frame &F = mb->frames[f];
+        MixedSixelFrame &D = desc[f];
+        const int w = F.out_w, h = (F.out_h + 5) / 6 * 6;
+        const long long npix = (long long)w * h;
+        long long step_px = npix / 18383; if (npix < 18383) step_px = 6; if (step_px == 0) step_px = 1;   // as sixel_plan
+        D.w = w; D.h = h;
+        D.ent_cap = (int)std::min<long long>(32768, (npix + step_px - 1) / step_px);
+        D.nb32 = (h + 31) / 32; D.nbands = h / 6;
+        D.fb_px = px; px += (unsigned long long)npix;
+        D.idx = idx; idx += align_up((size_t)npix, 16);
+        D.ent = ent; ent += (size_t)D.ent_cap;
+        D.bnd = bnd; bnd += (size_t)D.nb32 * w;
+        D.prog0 = (int)prog; prog += (size_t)D.nb32;
+        D.band_cap = align_up((size_t)w * 42 + 256 * 5 + 16, 256);
+        D.scr = scr; scr += D.band_cap * D.nbands;
+        D.band0 = (int)bands; band_start[f] = bands; bands += (unsigned)D.nbands;
+        D.cols_per_warp = ((w + EW - 1) / EW + 31) / 32 * 32;
+        int fw = 1;
+        const int per_frame = sixel_dither_split(D.nb32, n, ctx->sm_count, &D.bands_per_cta, &fw);
+        nwarps = std::max(nwarps, fw);
+        split |= per_frame > 1;
+        cta_start[f] = ctas; ctas += (unsigned)per_frame;
+        const size_t t_words = D.ent_cap > 16384 ? (size_t)D.ent_cap : 16384;
+        const size_t smem_tables = sizeof(uint32_t) * (t_words + (size_t)D.ent_cap);
+        if (smem_tables <= 200 * 1024) { list[0].push_back(f); pal_smem = std::max(pal_smem, smem_tables); }
+        else list[1].push_back(f);
+        wmax = std::max(wmax, w);
+    }
+    band_start[n] = bands; cta_start[n] = ctas;
+    mp.sixel_list[0] = (int)list[0].size(); mp.sixel_list[1] = (int)list[1].size();
+    for (auto &l : list) if (l.empty()) l.push_back(0);               // a launch without frames still reads list[0]
+    mp.o_sixel = mixed_put(mp.arena, desc.data(), sizeof(MixedSixelFrame) * n);
+    mp.o_sband = mixed_put(mp.arena, band_start.data(), sizeof(unsigned) * (n + 1));
+    mp.o_scta = mixed_put(mp.arena, cta_start.data(), sizeof(unsigned) * (n + 1));
+    mp.o_slist[0] = mixed_put(mp.arena, list[0].data(), sizeof(int) * list[0].size());
+    mp.o_slist[1] = mixed_put(mp.arena, list[1].data(), sizeof(int) * list[1].size());
+    mp.sixel_bands = bands; mp.sixel_ctas = ctas;
+    mp.sixel_nwarps = nwarps; mp.sixel_wmax = wmax; mp.sixel_split = split;
+    mp.sixel_pal_smem = pal_smem;
+    mp.sixel_ent = ent; mp.sixel_idx = idx; mp.sixel_bnd = bnd; mp.sixel_scr = scr; mp.sixel_prog = prog;
+    size_t o_bnd, o_prog;
+    B2_CUDA(ctx, ctx->sixel_work.reserve(mixed_sixel_work(mp, n, nullptr, nullptr, &o_bnd, &o_prog)));
+    return B200TIMG_OK;
+}
+
+int launch_sixel_mixed(b200timg_ctx *ctx, const MixedPlan &mp, const char *d_arena, const uint8_t *d_fb, int n,
+                       char *d_out, size_t out_cap, uint64_t *d_offsets) {
+    char *base = ctx->sixel_work.as<char>();
+    SixelWork W;
+    size_t o_bnd, o_prog;
+    mixed_sixel_work(mp, n, base, &W, &o_bnd, &o_prog);
+    ctx->sixel_idx_off = (size_t)(reinterpret_cast<char *>(W.index) - base);      // b200timg_sixel_debug: frame 0
+    const uint32_t *fb = reinterpret_cast<const uint32_t *>(d_fb);
+    MixedSixelParams M;
+    M.desc = reinterpret_cast<const MixedSixelFrame *>(d_arena + mp.o_sixel);
+    M.band_start = reinterpret_cast<const unsigned *>(d_arena + mp.o_sband);
+    M.cta_start = reinterpret_cast<const unsigned *>(d_arena + mp.o_scta);
+    M.n_frames = n; M.nwarps = mp.sixel_nwarps;
+    B2_CUDA(ctx, cudaFuncSetAttribute(sixel_palette_kernel<true, PaletteMixed>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    B2_CUDA(ctx, cudaFuncSetAttribute(sixel_palette_kernel<false, PaletteMixed>, cudaFuncAttributeMaxDynamicSharedMemorySize, 65536));
+    B2_CUDA(ctx, cudaFuncSetAttribute(sixel_emit1b_kernel<true, BandMixed>, cudaFuncAttributeMaxDynamicSharedMemorySize, (227 - 47) * 1024));
+    for (int k = 0; k < 2; ++k) {                 // every launch runs even without frames: the launch count stays fixed
+        M.list = reinterpret_cast<const int *>(d_arena + mp.o_slist[k]);
+        M.n_list = mp.sixel_list[k];
+        const unsigned grid = (unsigned)std::max(1, M.n_list);
+        B2_KERNEL(ctx, "sixel_palette_mixed_kernel");
+        if (k == 0) sixel_palette_kernel<true, PaletteMixed><<<grid, PT, std::max<size_t>(mp.sixel_pal_smem, 4), ctx->stream>>>(fb, 0, 0, W, M);
+        else sixel_palette_kernel<false, PaletteMixed><<<grid, PT, 65536, ctx->stream>>>(fb, 0, 0, W, M);
+        B2_LAUNCH_CHECK(ctx);
+    }
+    M.list = nullptr; M.n_list = 0;
+    B2_KERNEL(ctx, "sixel_lut_kernel");
+    sixel_lut_kernel<<<dim3(128, n), 256, 0, ctx->stream>>>(W);
+    B2_LAUNCH_CHECK(ctx);
+    B2_KERNEL(ctx, "sixel_map_mixed_kernel");
+    sixel_map_kernel<MapMixed><<<dim3(64, n), 256, 0, ctx->stream>>>(fb, 0, W, M);
+    B2_LAUNCH_CHECK(ctx);
+    B2_TRY(launch_sixel_dither_mixed(ctx, fb, mp.sixel_ctas, M, W, base + o_bnd, base + o_prog, mp.sixel_prog, mp.sixel_split != 0));
+    B2_KERNEL(ctx, "sixel_emit5_mixed_kernel");
+    sixel_emit1b_kernel<true, BandMixed><<<mp.sixel_bands, ET, sizeof(uint32_t) * (size_t)6 * mp.sixel_wmax, ctx->stream>>>(M, W);
+    B2_LAUNCH_CHECK(ctx);
+    B2_KERNEL(ctx, "sixel_layout_mixed_kernel");
+    sixel_layout_kernel<LayoutMixed><<<n, 256, 0, ctx->stream>>>(0, 0, W, M);
+    B2_LAUNCH_CHECK(ctx);
+    B2_KERNEL(ctx, "sixel_sizes_to_offsets_kernel");
+    sixel_sizes_to_offsets_kernel<<<1, 1024, 0, ctx->stream>>>(W.hdr, n, d_offsets);
+    B2_LAUNCH_CHECK(ctx);
+    B2_KERNEL(ctx, "sixel_compact_mixed_kernel");
+    sixel_compact_kernel<BandMixed><<<mp.sixel_bands, 256, 0, ctx->stream>>>(0, 0, W, d_offsets, d_out, (unsigned long long)out_cap, M);
+    B2_LAUNCH_CHECK(ctx);
+    return B200TIMG_OK;
 }
 
 // Introspection for tests: palette, colour counts and index plane of frame 0 of the last encode.

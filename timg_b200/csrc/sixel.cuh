@@ -29,6 +29,39 @@ struct SixelWork {                     // device pointers into ctx->sixel_work
     uint32_t *ctl;                     // [0] CTA ticket, [1] status (bit 0: output buffer too small)
 };
 
+// One frame of a mixed-geometry sixel batch (b200timg_sixel_mixed_dev): its padded geometry and where its parts live.
+// Offsets count elements from the bases in SixelWork (ent_a / ent_b, index, scratch) and from the dither's boundary and
+// progress arrays; headers and nearest-colour tables stay dense per frame (W.hdr + f, W.lut + f * 32768).
+struct __align__(16) MixedSixelFrame {
+    unsigned long long fb_px;          // first pixel of the padded frame in the scaled framebuffer
+    unsigned long long idx;            // first index byte
+    unsigned long long ent;            // first median-cut table entry
+    unsigned long long bnd;            // first boundary element of the dither (uint4)
+    unsigned long long scr;            // first scratch byte of band 0
+    unsigned long long band_cap;       // scratch bytes per band
+    int w, h, nb32, nbands, ent_cap;   // h: padded rows (a multiple of 6)
+    int band0, prog0;                  // first flat band (band_bytes / band_off) and first progress flag
+    int cols_per_warp, bands_per_cta;  // emit5's column split; the dither's bands per CTA
+};
+// What the mixed kernels read besides SixelWork: the descriptors and the flat item lists (all in ctx->mixed_arena).
+struct MixedSixelParams {
+    const MixedSixelFrame *desc;
+    const unsigned *band_start;        // [n + 1] first flat band of each frame (emit, compaction)
+    const unsigned *cta_start;         // [n + 1] first dither CTA of each frame
+    const int *list;                   // palette launch: the frames it covers
+    int n_frames, n_list, nwarps;      // nwarps: the dither launch's warps per CTA
+};
+
+// mixed batches: the frame that owns flat item `item`: the last f with start[f] <= item
+__device__ __forceinline__ int sixel_owner(const unsigned *__restrict__ start, int n, unsigned item) {
+    int lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (start[mid] <= item) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
 __device__ __forceinline__ uint32_t hash15(uint32_t px) {   // (r>>3)<<10 | (g>>3)<<5 | (b>>3)
     return ((px & 0xf8) << 7) | ((px >> 6) & 0x3e0) | ((px >> 19) & 0x1f);
 }
@@ -87,6 +120,9 @@ int launch_sixel_emit3(b200timg_ctx *ctx, int w, int h, int n_frames, const Sixe
                        uint64_t *d_offsets);
 size_t sixel_dither_workspace(int w, int h, int n_frames, size_t *o_bnd, size_t *o_prog);
 int launch_sixel_dither(b200timg_ctx *ctx, const uint32_t *fb, int w, int h, int n_frames, int n_total, const SixelWork &W, void *d_bnd, void *d_prog);
+int sixel_dither_split(int nb32, int n_frames, int sm_count, int *bands_per_cta, int *nwarps);
+int launch_sixel_dither_mixed(b200timg_ctx *ctx, const uint32_t *fb, unsigned n_ctas, const MixedSixelParams &M, const SixelWork &W,
+                              void *d_bnd, void *d_prog, size_t n_prog, bool split);
 size_t sixel_emit_workspace(int w, int h, int n_frames, size_t *o_hdr_bytes, size_t *o_desc, size_t *o_ctl);
 
 }  // namespace b200timg

@@ -58,17 +58,58 @@ __device__ __forceinline__ uint32_t add_clamp(uint32_t v, uint32_t t) { return _
 
 struct Dither2Geom { int w, h, nb32, bands_per_cta, nwarps; unsigned spin_ns; };   // spin_ns: pause between two polls of the band above
 
+// The CTA's frame and its part of the frame's bands (see sixel.cu's accessors):
+//   DitherUniform  CTA blockIdx.x of frame blockIdx.y, Dither2Geom's geometry for every frame
+//   DitherMixed    flat CTA blockIdx.x of a mixed batch; the block size (nwarps) is the launch's, a frame with fewer
+//                  bands than warps leaves the spare warps idle after the setup barrier
+struct DitherUniform {
+    typedef Dither2Geom Params;
+    const Dither2Geom &G; int f, g;
+    __device__ __forceinline__ explicit DitherUniform(const Dither2Geom &p) : G(p), f(blockIdx.y), g(blockIdx.x) {}
+    __device__ __forceinline__ int w() const { return G.w; }
+    __device__ __forceinline__ int h() const { return G.h; }
+    __device__ __forceinline__ int nb32() const { return G.nb32; }
+    __device__ __forceinline__ int bands_per_cta() const { return G.bands_per_cta; }
+    __device__ __forceinline__ int nwarps() const { return G.nwarps; }
+    __device__ __forceinline__ unsigned spin_ns() const { return G.spin_ns; }
+    __device__ __forceinline__ long long px0() const { return (long long)f * G.w * G.h; }
+    __device__ __forceinline__ long long idx0() const { return (long long)f * G.w * G.h; }
+    __device__ __forceinline__ long long bnd0() const { return (long long)f * G.nb32 * G.w; }
+    __device__ __forceinline__ long long prog0() const { return (long long)f * G.nb32; }
+};
+struct DitherMixed {
+    typedef MixedSixelParams Params;
+    MixedSixelFrame D; int f, g, nw;
+    __device__ __forceinline__ explicit DitherMixed(const MixedSixelParams &P) : nw(P.nwarps) {
+        f = sixel_owner(P.cta_start, P.n_frames, blockIdx.x);
+        g = (int)(blockIdx.x - P.cta_start[f]);
+        D = P.desc[f];
+    }
+    __device__ __forceinline__ int w() const { return D.w; }
+    __device__ __forceinline__ int h() const { return D.h; }
+    __device__ __forceinline__ int nb32() const { return D.nb32; }
+    __device__ __forceinline__ int bands_per_cta() const { return D.bands_per_cta; }
+    __device__ __forceinline__ int nwarps() const { return nw; }
+    __device__ __forceinline__ unsigned spin_ns() const { return 256; }     // the uniform default
+    __device__ __forceinline__ long long px0() const { return (long long)D.fb_px; }
+    __device__ __forceinline__ long long idx0() const { return (long long)D.idx; }
+    __device__ __forceinline__ long long bnd0() const { return (long long)D.bnd; }
+    __device__ __forceinline__ long long prog0() const { return (long long)D.prog0; }
+};
+
+template <class A>
 __global__ void __launch_bounds__(D2_WMAX * 32)
-sixel_dither2_kernel(const uint32_t *__restrict__ fb, Dither2Geom G, SixelWork W, uint4 *__restrict__ bnd_all, int *__restrict__ gprog_all) {
+sixel_dither2_kernel(const uint32_t *__restrict__ fb, typename A::Params G, SixelWork W, uint4 *__restrict__ bnd_all, int *__restrict__ gprog_all) {
     extern __shared__ __align__(16) uint8_t s_dyn2[];            // lut[32768] | per-warp tiles
     __shared__ uint2 s_pal2[256];                                // (256 - P) per half: .x = R | G << 16, .y = B | 256 << 16
     __shared__ uint32_t s_tap[512];                              // [e + 256] -> t7 | t3 << 8 | t5 << 16 | t1 << 24 (signed bytes)
     __shared__ volatile int s_progress[2048];             // columns completed by the last row of each band of this CTA
-    const int f = blockIdx.y, g = blockIdx.x;
+    const A a(G);
+    const int f = a.f, g = a.g;
     const SixelFrameHdr *hdr = W.hdr + f;
     if (!hdr->diffuse) return;
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    const int nthreads = G.nwarps * 32, w = G.w, h = G.h;
+    const int nthreads = a.nwarps() * 32, w = a.w(), h = a.h();
     uint8_t *s_lut = s_dyn2;
     for (int i = tid; i < 32768 / 16; i += nthreads)
         reinterpret_cast<uint4 *>(s_lut)[i] = reinterpret_cast<const uint4 *>(W.lut + (long long)f * 32768)[i];
@@ -81,28 +122,28 @@ sixel_dither2_kernel(const uint32_t *__restrict__ fb, Dither2Geom G, SixelWork W
         const int t7 = e * 7 / 16, t3 = e * 3 / 16, t5 = e * 5 / 16, t1 = e / 16;          // C truncation (error_diffuse)
         s_tap[i] = (uint32_t)(t7 & 0xff) | ((uint32_t)(t3 & 0xff) << 8) | ((uint32_t)(t5 & 0xff) << 16) | ((uint32_t)(t1 & 0xff) << 24);
     }
-    const int band_lo = g * G.bands_per_cta, band_hi = min(G.nb32, band_lo + G.bands_per_cta);
+    const int band_lo = g * a.bands_per_cta(), band_hi = min(a.nb32(), band_lo + a.bands_per_cta());
     const int nlocal = band_hi - band_lo;
     for (int i = tid; i < nlocal; i += nthreads) s_progress[i] = 0;
     __syncthreads();
     uint32_t *s_in = reinterpret_cast<uint32_t *>(s_dyn2 + 32768 + (size_t)wid * D2_WARP_SMEM);   // [2][32][D2_IN_STRIDE]
     uint8_t *s_out = reinterpret_cast<uint8_t *>(s_in + 2 * 32 * D2_IN_STRIDE);                    // [32][D2_OUT_STRIDE]
     uint4 *s_bnd = reinterpret_cast<uint4 *>(s_out + 32 * D2_OUT_STRIDE);                          // [D2_CH]
-    const uint32_t *frame = fb + (long long)f * w * h;
-    uint8_t *index = W.index + (long long)f * w * h;
-    uint4 *bnd = bnd_all + (long long)f * G.nb32 * w;
-    volatile int *gprog = gprog_all + (long long)f * G.nb32;
+    const uint32_t *frame = fb + a.px0();
+    uint8_t *index = W.index + a.idx0();
+    uint4 *bnd = bnd_all + a.bnd0();
+    volatile int *gprog = gprog_all + a.prog0();
     const int hrow = lane >> 4, hcol = lane & 15;                // half-warp staging coordinates (odd widths)
     const int qrow = lane >> 3, qcol = lane & 7;                 // quarter-warp staging coordinates (even widths: pixel pairs)
     const bool even_w = (w & 1) == 0;
     const TapW Z = {0u, 0u, 0u};
 
-    for (int band = band_lo + wid; band < band_hi; band += G.nwarps) {
+    for (int band = band_lo + wid; band < band_hi; band += a.nwarps()) {
         const int lb = band - band_lo;
         const int y = band * 32 + lane;
         const bool row_ok = y < h, last_row = (y == h - 1);
         const bool prev_remote = band > 0 && lb == 0;            // the band above belongs to another CTA
-        const bool publish_remote = band + 1 < G.nb32 && band + 1 == band_hi;
+        const bool publish_remote = band + 1 < a.nb32() && band + 1 == band_hi;
         const uint4 *bin = band > 0 ? bnd + (long long)(band - 1) * w : nullptr;
         uint4 *bout = bnd + (long long)band * w;
         TapW own = Z, a0 = Z, a1 = Z, a2 = Z, e_first = Z;
@@ -148,8 +189,8 @@ sixel_dither2_kernel(const uint32_t *__restrict__ fb, Dither2Geom G, SixelWork W
             if (band > 0) {                                      // stay behind the band above's last row
                 const int need = min(w, t0 + D2_CH + 1);
                 if (lane == 0) {
-                    if (prev_remote) { while (gprog[band - 1] < need) __nanosleep(G.spin_ns); __threadfence(); }
-                    else { while (s_progress[lb - 1] < need) __nanosleep(G.spin_ns); __threadfence_block(); }
+                    if (prev_remote) { while (gprog[band - 1] < need) __nanosleep(a.spin_ns()); __threadfence(); }
+                    else { while (s_progress[lb - 1] < need) __nanosleep(a.spin_ns()); __threadfence_block(); }
                 }
                 __syncwarp();
                 const int bx = t0 + 1 + lane;                    // lane 0 consumes column t+1 at step t
@@ -281,10 +322,34 @@ int launch_sixel_dither(b200timg_ctx *ctx, const uint32_t *fb, int w, int h, int
     G.nwarps = (G.bands_per_cta + rounds - 1) / rounds;
     if (G.bands_per_cta > 2048) return ctx->fail(B200TIMG_EINVAL, "sixel: frame too tall");
     const size_t smem = 32768 + (size_t)G.nwarps * D2_WARP_SMEM;
-    B2_CUDA(ctx, cudaFuncSetAttribute(sixel_dither2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 32768 + D2_WMAX * D2_WARP_SMEM));
+    B2_CUDA(ctx, cudaFuncSetAttribute(sixel_dither2_kernel<DitherUniform>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32768 + D2_WMAX * D2_WARP_SMEM));
     if (per_frame > 1) B2_CUDA(ctx, cudaMemsetAsync(d_prog, 0, sizeof(int) * (size_t)G.nb32 * n_frames, ctx->stream));
     B2_KERNEL(ctx, "sixel_dither2_kernel");
-    sixel_dither2_kernel<<<dim3(per_frame, n_frames), G.nwarps * 32, smem, ctx->stream>>>(fb, G, W, static_cast<uint4 *>(d_bnd), static_cast<int *>(d_prog));
+    sixel_dither2_kernel<DitherUniform><<<dim3(per_frame, n_frames), G.nwarps * 32, smem, ctx->stream>>>(fb, G, W, static_cast<uint4 *>(d_bnd), static_cast<int *>(d_prog));
+    B2_LAUNCH_CHECK(ctx);
+    return B200TIMG_OK;
+}
+
+// Mixed batches: launch_sixel_dither's default split for one frame of nb32 bands in a batch of n_frames.  A frame is split
+// only when the batch has fewer frames than SMs, and then into at most sm_count / n_frames CTAs, so that every CTA of the
+// launch can be resident at once.  Returns the frame's CTAs; *bands_per_cta and *nwarps (the warps it would run with).
+int sixel_dither_split(int nb32, int n_frames, int sm_count, int *bands_per_cta, int *nwarps) {
+    int per_frame = 1;
+    if (n_frames < sm_count) per_frame = std::max(1, std::min(sm_count / n_frames, (nb32 + 7) / 8));
+    *bands_per_cta = (nb32 + per_frame - 1) / per_frame;
+    const int rounds = (*bands_per_cta + D2_WMAX - 1) / D2_WMAX;
+    *nwarps = (*bands_per_cta + rounds - 1) / rounds;
+    return (nb32 + *bands_per_cta - 1) / *bands_per_cta;
+}
+
+// One launch over every frame's dither CTAs (M.cta_start); the block size is the largest any frame asks for.
+int launch_sixel_dither_mixed(b200timg_ctx *ctx, const uint32_t *fb, unsigned n_ctas, const MixedSixelParams &M, const SixelWork &W,
+                              void *d_bnd, void *d_prog, size_t n_prog, bool split) {
+    const size_t smem = 32768 + (size_t)M.nwarps * D2_WARP_SMEM;
+    B2_CUDA(ctx, cudaFuncSetAttribute(sixel_dither2_kernel<DitherMixed>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32768 + D2_WMAX * D2_WARP_SMEM));
+    if (split) B2_CUDA(ctx, cudaMemsetAsync(d_prog, 0, sizeof(int) * n_prog, ctx->stream));
+    B2_KERNEL(ctx, "sixel_dither2_mixed_kernel");
+    sixel_dither2_kernel<DitherMixed><<<n_ctas, M.nwarps * 32, smem, ctx->stream>>>(fb, M, W, static_cast<uint4 *>(d_bnd), static_cast<int *>(d_prog));
     B2_LAUNCH_CHECK(ctx);
     return B200TIMG_OK;
 }

@@ -1,20 +1,23 @@
 #!/usr/bin/env python
-"""Mixed batches on the GPU: a `timg --grid` page of differently sized images, block-encoded in one call
-(b200timg_blocks_mixed_dev) against the ways to send it without one.  One JSON line per page.
+"""Mixed batches on the GPU: a `timg --grid` page of differently sized images, block- or sixel-encoded in one call
+(b200timg_blocks_mixed_dev, b200timg_sixel_mixed_dev) against the ways to send it without one.  One JSON line per page.
 
   python tools/bench_mixed.py [--steps K] [--warmup W] [--only NAME]
 
   grid8x8-quarter  --grid=8x8 -g300x100 -p quarter: 64 images, each fitted to the grid's 75 x 25 px box
   grid4x4-half     --grid=4x4 -g300x100 -p half: 16 images fitted to 75 x 50 px (larger outputs per image)
+  grid4x4-sixel    --grid=4x4 -g300x100 -p sixel at 9 x 18 px cells: 16 images fitted to 675 x 450 px
+  grid8x8-sixel    --grid=8x8 -g300x100 -p sixel at 9 x 18 px cells: 64 images fitted to 337 x 225 px
 Source sizes cycle through 3840x2160, 2160x3840, 4032x3024, 3000x2000, 1920x1080, 1280x720, 1080x1080 and 640x480
 (every image's pixels distinct); indents are the renderer's column offsets (src/renderer.cc:124-142).
 
 Timed, alternating within each step, every call ending in a device-wide synchronise:
-  (a) mixed     one b200timg_blocks_mixed_dev call for the page
-  (b) per_image one b200timg_blocks_batch_dev call per image (n_frames = 1): the status quo
-  (c) per_geom  one uniform b200timg_blocks_batch_dev call per distinct geometry (sources regrouped by geometry)
+  (a) mixed     one b200timg_blocks_mixed_dev (sixel pages: b200timg_sixel_mixed_dev) call for the page
+  (b) per_image one b200timg_blocks_batch_dev (b200timg_sixel_batch_dev) call per image (n_frames = 1): the status quo
+  (c) per_geom  one uniform batch call per distinct geometry (sources regrouped by geometry)
   (d) the cost of generality: C3 geometry (1920x1080 -> 320x90, -p quarter, 64 frames) through the mixed call against
-      b200timg_blocks_batch_dev
+      b200timg_blocks_batch_dev, and C4's (3840x2160 -> 337x190, -p sixel, 64 frames) through the sixel mixed call
+      against b200timg_sixel_batch_dev with flags = 0
 (a), (b) and (c) must produce the same bytes for every image (asserted); so must both sides of (d).  Per-kernel ms of one
 (a) and one (b) page come from b200timg_profile in a separate run.  The GPU's name, power limit and max SM clock are read
 in the same run.
@@ -39,6 +42,8 @@ SIZES = [(3840, 2160), (2160, 3840), (4032, 3024), (3000, 2000), (1920, 1080), (
 PAGES = {
     "grid8x8-quarter": dict(cols=8, rows=8, term=(300, 100), quarter=True),
     "grid4x4-half": dict(cols=4, rows=4, term=(300, 100), quarter=False),
+    "grid4x4-sixel": dict(cols=4, rows=4, term=(300, 100), quarter=False, sixel=True),
+    "grid8x8-sixel": dict(cols=8, rows=8, term=(300, 100), quarter=False, sixel=True),
 }
 
 
@@ -53,7 +58,7 @@ def gpu_info():
 
 def page_layout(cfg):
     """(images' source sizes, fitted outputs, indents) of one page, as timg.cc:938-939 and renderer.cc lay it out."""
-    cx, cy = (2, 2) if cfg["quarter"] else (1, 2)
+    cx, cy = (9, 18) if cfg.get("sixel") else (2, 2) if cfg["quarter"] else (1, 2)
     box_w = cfg["term"][0] * cx // cfg["cols"]
     box_h = cfg["term"][1] * cy // cfg["rows"]
     n = cfg["cols"] * cfg["rows"]
@@ -63,7 +68,7 @@ def page_layout(cfg):
         _, ow, oh = timg_b200.calc_fit(iw, ih, box_w, box_h, cx, cy)
         srcs.append((iw, ih))
         outs.append((ow, oh))
-        indents.append((i % cfg["cols"]) * box_w // cx)     # UnicodeBlockCanvas::Send's x / cell_x_px
+        indents.append(0 if cfg.get("sixel") else (i % cfg["cols"]) * box_w // cx)   # UnicodeBlockCanvas::Send's x / cell_x_px
     return srcs, outs, indents
 
 
@@ -96,9 +101,18 @@ def timed(torch, fn, steps):
     return (time.perf_counter() - t0) * 1e3 / steps
 
 
+def encoder(L, sixel):
+    """(mixed call, uniform batch call, per-frame staging bound) of the block or the sixel encoder."""
+    if sixel:
+        return (L.b200timg_sixel_mixed_dev, L.b200timg_sixel_batch_dev,
+                lambda ow, oh: L.b200timg_sixel_bound(ow, (oh + 5) // 6 * 6))
+    return L.b200timg_blocks_mixed_dev, L.b200timg_blocks_batch_dev, L.b200timg_blocks_bound
+
+
 def run_page(name, cfg, steps, warmup, torch):
     L = timg_b200.lib()
     ctx = timg_b200.Context(0)
+    mixed_fn, batch_fn, bound_fn = encoder(L, cfg.get("sixel", False))
     flags = timg_b200.QUARTER if cfg["quarter"] else 0
     bg = timg_b200.rgba_u32(0, 0, 0)
     srcs, outs, indents = page_layout(cfg)
@@ -107,7 +121,7 @@ def run_page(name, cfg, steps, warmup, torch):
     flat, offs = pack(torch, imgs)
     torch.cuda.synchronize()                   # sources are written on torch's stream, read on the context's
     mb, keep = timg_b200.mixed_batch([(h, w) for w, h in srcs], outs, offs, indents, flags, has_bg=True, bg=bg)
-    bounds = [L.b200timg_blocks_bound(ow, oh) for ow, oh in outs]
+    bounds = [bound_fn(ow, oh) for ow, oh in outs]
     cap = sum(bounds)
     d_out_a = torch.empty(cap, dtype=torch.uint8, device="cuda")
     d_offs_a = torch.empty(n + 1, dtype=torch.int64, device="cuda")
@@ -117,7 +131,7 @@ def run_page(name, cfg, steps, warmup, torch):
                                pattern_w=0, pattern_h=0, flags=flags, x_indent_cells=indent, animation=0)
 
     def run_a():
-        ctx._chk(L.b200timg_blocks_mixed_dev(ctx.h, C.byref(mb), flat.data_ptr(), d_out_a.data_ptr(), cap, d_offs_a.data_ptr()))
+        ctx._chk(mixed_fn(ctx.h, C.byref(mb), flat.data_ptr(), d_out_a.data_ptr(), cap, d_offs_a.data_ptr()))
 
     # (b): one call per image, image i's bytes in its own slot
     slot = np.cumsum([0] + bounds)
@@ -127,8 +141,8 @@ def run_page(name, cfg, steps, warmup, torch):
 
     def run_b():
         for i in range(n):
-            ctx._chk(L.b200timg_blocks_batch_dev(ctx.h, C.byref(b_batches[i]), flat.data_ptr() + offs[i],
-                                                 d_out_b.data_ptr() + int(slot[i]), bounds[i], d_offs_b[i].data_ptr()))
+            ctx._chk(batch_fn(ctx.h, C.byref(b_batches[i]), flat.data_ptr() + offs[i],
+                              d_out_b.data_ptr() + int(slot[i]), bounds[i], d_offs_b[i].data_ptr()))
 
     # (c): images regrouped by geometry; one uniform call per geometry (the indent is per call, so frames of a group
     # that sit in different columns would need one call each: the bytes are compared with indents folded in below)
@@ -142,7 +156,7 @@ def run_page(name, cfg, steps, warmup, torch):
     c_calls, pos = [], 0
     for (src, out, indent), members in geoms.items():
         k = len(members)
-        gcap = k * L.b200timg_blocks_bound(*out)
+        gcap = k * bound_fn(*out)
         c_calls.append((batch(src[0], src[1], out[0], out[1], k, indent), offs_c[pos], gcap,
                         torch.empty(k + 1, dtype=torch.int64, device="cuda"), members))
         pos += k
@@ -150,8 +164,7 @@ def run_page(name, cfg, steps, warmup, torch):
 
     def run_c():
         for j, (b, o, gcap, d_o, _) in enumerate(c_calls):
-            ctx._chk(L.b200timg_blocks_batch_dev(ctx.h, C.byref(b), flat_c.data_ptr() + o, d_out_c.data_ptr() + int(c_base[j]),
-                                                 gcap, d_o.data_ptr()))
+            ctx._chk(batch_fn(ctx.h, C.byref(b), flat_c.data_ptr() + o, d_out_c.data_ptr() + int(c_base[j]), gcap, d_o.data_ptr()))
 
     for _ in range(warmup):
         run_a(); run_b(); run_c()
@@ -198,11 +211,18 @@ def run_page(name, cfg, steps, warmup, torch):
     return res
 
 
-def run_generality(steps, warmup, torch):
-    """(d): C3 geometry through the mixed call and through the uniform batch."""
+GENERALITY = {
+    "C3-generality": dict(iw=1920, ih=1080, ow=320, oh=90, flags=timg_b200.QUARTER, sixel=False),
+    "C4-generality": dict(iw=3840, ih=2160, ow=337, oh=190, flags=0, sixel=True),
+}
+
+
+def run_generality(name, g, steps, warmup, torch):
+    """(d): one geometry through the mixed call and through the uniform batch."""
     L = timg_b200.lib()
     ctx = timg_b200.Context(0)
-    n, iw, ih, ow, oh, indent = 64, 1920, 1080, 320, 90, 0
+    mixed_fn, batch_fn, bound_fn = encoder(L, g["sixel"])
+    n, iw, ih, ow, oh, indent, flags = 64, g["iw"], g["ih"], g["ow"], g["oh"], 0, g["flags"]
     bg = timg_b200.rgba_u32(0, 0, 0)
     base = synth.frame_torch(800, iw, ih, "photo")
     d_src = torch.empty((n, ih, iw, 4), dtype=torch.uint8, device="cuda")
@@ -211,19 +231,19 @@ def run_generality(steps, warmup, torch):
         d_src[f, ..., :3] += (37 * f + 1) & 255
     fbytes = iw * ih * 4
     mb, keep = timg_b200.mixed_batch([(ih, iw)] * n, [(ow, oh)] * n, [f * fbytes for f in range(n)], [indent] * n,
-                                     timg_b200.QUARTER, has_bg=True, bg=bg)
+                                     flags, has_bg=True, bg=bg)
     ub = timg_b200.Batch(n_frames=n, src_w=iw, src_h=ih, src_fmt=0, out_w=ow, out_h=oh, has_bg=1, bg=bg, pattern=0, pattern_w=0,
-                         pattern_h=0, flags=timg_b200.QUARTER, x_indent_cells=indent, animation=0)
-    cap = n * L.b200timg_blocks_bound(ow, oh)
+                         pattern_h=0, flags=flags, x_indent_cells=indent, animation=0)
+    cap = n * bound_fn(ow, oh)
     outs = [torch.empty(cap, dtype=torch.uint8, device="cuda") for _ in range(2)]
     offs = [torch.empty(n + 1, dtype=torch.int64, device="cuda") for _ in range(2)]
     torch.cuda.synchronize()
 
     def mixed():
-        ctx._chk(L.b200timg_blocks_mixed_dev(ctx.h, C.byref(mb), d_src.data_ptr(), outs[0].data_ptr(), cap, offs[0].data_ptr()))
+        ctx._chk(mixed_fn(ctx.h, C.byref(mb), d_src.data_ptr(), outs[0].data_ptr(), cap, offs[0].data_ptr()))
 
     def uniform():
-        ctx._chk(L.b200timg_blocks_batch_dev(ctx.h, C.byref(ub), d_src.data_ptr(), outs[1].data_ptr(), cap, offs[1].data_ptr()))
+        ctx._chk(batch_fn(ctx.h, C.byref(ub), d_src.data_ptr(), outs[1].data_ptr(), cap, offs[1].data_ptr()))
     for _ in range(warmup):
         mixed(); uniform()
     tm = tu = 0.0
@@ -232,7 +252,7 @@ def run_generality(steps, warmup, torch):
         tu += timed(torch, uniform, 1)
     tm, tu = tm / steps, tu / steps
     same = bool((offs[0] == offs[1]).all()) and bool((outs[0][:int(offs[0][-1])] == outs[1][:int(offs[1][-1])]).all())
-    assert same, "mixed call differs from the uniform batch on C3 geometry"
+    assert same, f"mixed call differs from the uniform batch ({name})"
     kernels = {}
     for key, fn in (("mixed", mixed), ("uniform", uniform)):
         ctx.profile(True)
@@ -240,7 +260,7 @@ def run_generality(steps, warmup, torch):
         kernels[key] = {k: [v[0], round(v[1], 4)] for k, v in ctx.profile_report().items()}
         ctx.profile(False)
     ctx.close()
-    return dict(page="C3-generality", frames=n, src=f"{iw}x{ih}", out=f"{ow}x{oh}", steps=steps, same_bytes=same,
+    return dict(page=name, frames=n, src=f"{iw}x{ih}", out=f"{ow}x{oh}", steps=steps, same_bytes=same,
                 mixed_ms=round(tm, 3), uniform_ms=round(tu, 3), mixed_over_uniform=round(tm / tu, 2),
                 mixed_mpx_s=round(n * iw * ih / tm / 1e3, 1), uniform_mpx_s=round(n * iw * ih / tu / 1e3, 1),
                 kernels_ms_mixed=kernels["mixed"], kernels_ms_uniform=kernels["uniform"])
@@ -261,10 +281,13 @@ def main():
         r["gpu"] = info
         print(json.dumps(r), flush=True)
         torch.cuda.empty_cache()
-    if not a.only or a.only == "C3-generality":
-        r = run_generality(a.steps, a.warmup, torch)
+    for name, g in GENERALITY.items():
+        if a.only and a.only != name:
+            continue
+        r = run_generality(name, g, a.steps, a.warmup, torch)
         r["gpu"] = info
         print(json.dumps(r), flush=True)
+        torch.cuda.empty_cache()
 
 
 if __name__ == "__main__":
