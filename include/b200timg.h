@@ -171,7 +171,9 @@ int b200timg_blocks_encode(b200timg_ctx *ctx, const uint8_t *fb, int w, int h,
 
 /* Worst-case encoded size of one sixel frame of w x h (h a multiple of 6).
  * Size limits of the sixel path (the reference has none; both are far beyond any terminal): w <= 99999 and
- * h <= 65536.  Frames up to 4095 px wide take the fast emit kernel, wider ones a column-tiled one. */
+ * h <= 65536 (with h a multiple of 6: 65532).  Every sixel entry point rejects a larger frame with B200TIMG_EINVAL and
+ * a message naming the limit before it launches anything.  Frames up to 4095 px wide take the fast emit kernel, wider
+ * ones a column-tiled one ((w + 4095) / 4096 tiles); b200timg_sixel_shape_of reports which. */
 size_t b200timg_sixel_bound(int w, int h);
 
 /* What libsixel does inside SixelCanvas::Send (src/sixel-canvas.cc:134-148):
@@ -215,6 +217,9 @@ typedef struct {
  * OUTPUT CAPACITY CONTRACT: the call cannot fail with B200TIMG_ENOSPC because it never learns the sizes on the
  * host.  d_offsets is always complete and exact (d_offsets[n_frames] = the bytes the batch needs); a frame whose
  * end would lie beyond out_cap is NOT written (nothing is ever written out of bounds, earlier frames are intact).
+ * One exception in degree: sixel frames wider than 4095 px go through a single-pass emitter that places every band and
+ * column tile on its own, so of the FIRST frame that does not fit, the pieces that end before out_cap may be written
+ * (with the bytes a large enough buffer gets); still nothing at or beyond out_cap, and the offsets are exact.
  * The caller therefore either passes out_cap >= n_frames * b200timg_{blocks,sixel}_bound(out_w, padded out_h)
  * (cannot overflow) or compares d_offsets[n_frames] with out_cap when it reads the offsets, and repeats the call
  * with a larger buffer if it is greater -- exactly what the host variants do internally. */
@@ -330,6 +335,24 @@ int b200timg_sixel_debug(b200timg_ctx *ctx, uint32_t *palette, uint32_t *counts,
 int b200timg_resample_plan(int in_w, int in_h, int out_w, int out_h, int axis, int *widest,
                            int *flags, int32_t *first, int32_t *count, int32_t *lead,
                            float *coeff, size_t coeff_cap);
+
+/* Host-only introspection of the launch shapes behind the sixel entry points (no GPU needed): what the library would
+ * launch for n_frames frames of w x h that are a slice of a batch of n_total frames (n_total == n_frames for a whole
+ * batch; b200timg_sixel_encode is a batch of one) on a device with sm_count multiprocessors.  Computed by the functions
+ * the launches call, the environment switches they honour included (B200TIMG_DITHER_SPLIT, B200TIMG_DITHER_WARPS,
+ * B200TIMG_EMIT).  Returns B200TIMG_EINVAL for a geometry the launch rejects (h not a multiple of 6, w > 99999,
+ * h > 65536, more than 65535 frames) and for out == NULL, sm_count <= 0, n_frames <= 0 or n_total < n_frames. */
+typedef struct {
+    int step_px, ent_cap, palette_global;      /* palette: sampling step, entries per median-cut table (<= 32768),
+                                                  1 = tables in global memory (more than 25600 entries), 0 = shared */
+    int nb32, dither_ctas, bands_per_cta, dither_warps, dither_rounds;
+                                               /* dither: bands of 32 rows, CTAs per frame (> 1 only for batches of fewer
+                                                  frames than SMs: min(sm_count / n_total, (nb32 + 7) / 8)), bands per
+                                                  CTA, warps per CTA (<= 24), rounds of a warp over its CTA's bands */
+    int emit_mode, emit_tiles, tile_w;         /* emit: 1/4/5 band scratch + compaction (5 up to 4095 px), 2/3 single
+                                                  pass; their column tiles ((w + 4095) / 4096) and a tile's width */
+} b200timg_sixel_shape;
+int b200timg_sixel_shape_of(int w, int h, int n_frames, int n_total, int sm_count, b200timg_sixel_shape *out);
 
 /* ======================= geometry passes around the path (SURVEY 8f rank 3, row a15) ===============
  * ApplyExifOp (src/jpeg-source.cc:84-119): mirror each row, then rotate by 0, 180, 90 or -90 degrees exactly as

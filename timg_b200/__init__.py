@@ -61,6 +61,11 @@ class Frame(C.Structure):
                 ("x_indent_cells", C.c_int)]
 
 
+class SixelShape(C.Structure):
+    _fields_ = [(k, C.c_int) for k in ("step_px", "ent_cap", "palette_global", "nb32", "dither_ctas", "bands_per_cta",
+                                       "dither_warps", "dither_rounds", "emit_mode", "emit_tiles", "tile_w")]
+
+
 class MixedBatch(C.Structure):
     _fields_ = [("n_frames", C.c_int), ("src_fmt", C.c_int), ("flags", C.c_int), ("has_bg", C.c_int), ("bg", C.c_uint32),
                 ("pattern", C.c_uint32), ("pattern_w", C.c_int), ("pattern_h", C.c_int), ("frames", C.POINTER(Frame))]
@@ -137,6 +142,7 @@ ABI = {
     "b200timg_sixel_debug": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     "b200timg_resample_plan": (C.c_int, [C.c_int] * 5 + [C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p,
                                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "b200timg_sixel_shape_of": (C.c_int, [C.c_int] * 5 + [C.POINTER(SixelShape)]),
 }
 
 _lib = None
@@ -200,6 +206,16 @@ def resample_plan(iw, ih, ow, oh, axis):
         raise B200Error(rc, "resample_plan")
     return dict(widest=widest.value, flags=flags.value, first=first, count=count, lead=lead,
                 coeff=coeff.reshape(n, widest.value))
+
+
+def sixel_shape(w, h, n_frames=1, n_total=None, sm_count=132):
+    """Host-side launch shape of the sixel kernels for n_frames frames of w x h out of a batch of n_total (default: the
+    whole batch) on a device with sm_count SMs, as a dict of b200timg_sixel_shape's fields (see include/b200timg.h)."""
+    s = SixelShape()
+    rc = lib().b200timg_sixel_shape_of(w, h, n_frames, n_frames if n_total is None else n_total, sm_count, C.byref(s))
+    if rc != OK:
+        raise B200Error(rc, f"sixel_shape: {w} x {h}, {n_frames} frames: not a geometry the sixel path takes")
+    return {k: getattr(s, k) for k, _ in SixelShape._fields_}
 
 
 def graphics(protocol, rgb24=False, ids=None, cell=None, indent=0):

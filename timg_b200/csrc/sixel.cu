@@ -1207,21 +1207,58 @@ struct SixelPlan {
     bool emit_v1, dither_v1;
     int emit_mode;                            // 1: v1, 4: v1b, 5: emit5 (scratch arena + compaction), 2: emit2, 3: emit3
     EmitGeom G;
+    SixelPaletteShape pal;
     size_t emit_smem, o_d2_bnd, o_d2_prog;
     long long npix;
 };
 
+int sixel_check_geometry(int w, int h, int n_frames, char *msg, size_t msg_cap) {
+    msg[0] = 0;
+    if (w <= 0 || h <= 0 || n_frames <= 0) snprintf(msg, msg_cap, "sixel: bad geometry %d x %d, %d frames", w, h, n_frames);
+    else if (h % 6) snprintf(msg, msg_cap, "sixel: height %d is not a multiple of 6", h);
+    else if (n_frames > 65535) snprintf(msg, msg_cap, "sixel: %d frames, at most 65535 in one launch", n_frames);
+    else if (w > 99999) snprintf(msg, msg_cap, "sixel: width %d, at most 99999 px", w);
+    else if ((h + 31) / 32 > 2048) snprintf(msg, msg_cap, "sixel: height %d, at most 65536 rows", h);
+    else if ((unsigned long long)n_frames * (h / 6) * ((w + 4095) / 4096) > 0x7fffffffull)
+        snprintf(msg, msg_cap, "sixel: more than 2^31 - 1 bands x column tiles in one launch");
+    return msg[0] ? B200TIMG_EINVAL : B200TIMG_OK;
+}
+
+SixelPaletteShape sixel_palette_shape(long long npix) {
+    SixelPaletteShape P;
+    // quant.c computeHistogram, QUALITY_LOW (the palette kernel computes the same step)
+    P.step_px = npix / 18383; if (npix < 18383) P.step_px = 6; if (P.step_px == 0) P.step_px = 1;
+    const long long ns = (npix + P.step_px - 1) / P.step_px;
+    P.ent_cap = (int)std::min<long long>(32768, ns);
+    const size_t t_words = P.ent_cap > 16384 ? (size_t)P.ent_cap : 16384;      // the histogram aliases the second table
+    P.tables_smem = sizeof(uint32_t) * (t_words + (size_t)P.ent_cap);
+    P.smem_tables = P.tables_smem <= 200 * 1024;
+    return P;
+}
+
+// The emitters (B200TIMG_EMIT=1..5): v1, v1b (4) and emit5 (5, the default up to 4095 px) write per-band bytes into a
+// scratch arena for the compaction kernel; emit2 (sixel_emit.cu: single pass, any width -- what wider frames get) and
+// emit3 (v1's sort + entry-parallel formatting + look-back placement; slower than v1 on C2 frames) place their own.
+// Every mode but the default is kept for A/B runs.
+int sixel_emit_mode(int w) {
+    const bool v1_fits = w <= 4095 && sizeof(uint32_t) * (size_t)6 * w <= (size_t)(227 - 36) * 1024;
+    const bool v1b_fits = w <= 4095 && sizeof(uint32_t) * (size_t)6 * w <= (size_t)(227 - 47) * 1024;
+    int mode = v1b_fits ? 5 : v1_fits ? 1 : 2;           // 5 = emit5 (v1b with staged rows and a coalesced copy-out)
+    if (getenv("B200TIMG_EMIT_V2")) mode = 2;
+    if (const char *e = getenv("B200TIMG_EMIT")) mode = atoi(e);
+    if (mode < 1 || mode > 5 || (mode == 1 && !v1_fits) || (mode >= 4 && !v1b_fits)) mode = 2;
+    return mode;
+}
+
 static int sixel_plan(b200timg_ctx *ctx, int w, int h, int n_frames, bool reserve, SixelPlan *S) {
-    if (h % 6) return ctx->fail(B200TIMG_EINVAL, "sixel: height %d is not a multiple of 6", h);
-    if (n_frames > 65535) return ctx->fail(B200TIMG_EINVAL, "sixel: too many frames for one launch");
+    char why[96];
+    if (sixel_check_geometry(w, h, n_frames, why, sizeof why) != B200TIMG_OK) return ctx->fail(B200TIMG_EINVAL, "%s", why);
     SixelWork &W = S->W;
     const long long npix = (long long)w * h;
     S->npix = npix;
-    long long step_px = npix / 18383; if (npix < 18383) step_px = 6; if (step_px == 0) step_px = 1;
-    const long long ns = (npix + step_px - 1) / step_px;
-    W.ent_cap = (int)std::min<long long>(32768, ns);
+    S->pal = sixel_palette_shape(npix);
+    W.ent_cap = S->pal.ent_cap;
     W.nb32 = (h + 31) / 32; W.nbands = h / 6;
-    if (W.nb32 > 2048) return ctx->fail(B200TIMG_EINVAL, "sixel: frame too tall");
     // workspace carve-up
     size_t off = 0;
     const size_t o_hdr = off; off += align_up(sizeof(SixelFrameHdr) * n_frames, 256);
@@ -1235,20 +1272,8 @@ static int sixel_plan(b200timg_ctx *ctx, int w, int h, int n_frames, bool reserv
     // worst case of one band: <= 6 entries per column, <= 7 bytes each ("!nnnn?" + char), "$#ccc" per colour
     W.band_cap = align_up((size_t)w * 42 + 256 * 5 + 16, 256);
     const size_t o_scr = off;
-    // the emitters (B200TIMG_EMIT=1..5): v1, v1b (4) and emit5 (5, the default up to 4095 px) write per-band bytes into a
-    // scratch arena for the compaction kernel; emit2 (sixel_emit.cu: single pass, any width -- what wider frames get) and
-    // emit3 (v1's sort + entry-parallel formatting + look-back placement; slower than v1 on C2 frames) place their own.
-    // Every mode but the default is kept for A/B runs.
-    {
-        const bool v1_fits = w <= 4095 && sizeof(uint32_t) * (size_t)6 * w <= (size_t)(227 - 36) * 1024;
-        const bool v1b_fits = w <= 4095 && sizeof(uint32_t) * (size_t)6 * w <= (size_t)(227 - 47) * 1024;
-        int mode = v1b_fits ? 5 : v1_fits ? 1 : 2;           // 5 = emit5 (v1b with staged rows and a coalesced copy-out)
-        if (getenv("B200TIMG_EMIT_V2")) mode = 2;
-        if (const char *e = getenv("B200TIMG_EMIT")) mode = atoi(e);
-        if (mode < 1 || mode > 5 || (mode == 1 && !v1_fits) || (mode >= 4 && !v1b_fits)) mode = 2;
-        S->emit_mode = mode;
-        S->emit_v1 = mode == 1 || mode >= 4;
-    }
+    S->emit_mode = sixel_emit_mode(w);
+    S->emit_v1 = S->emit_mode == 1 || S->emit_mode >= 4;
     if (S->emit_v1) off += W.band_cap * W.nbands * n_frames;
     S->dither_v1 = getenv("B200TIMG_DITHER_V1") != nullptr;      // round-1 ditherer, kept for A/B runs
     size_t d_bnd, d_prog;
@@ -1298,12 +1323,8 @@ int launch_sixel_front(b200timg_ctx *ctx, const uint8_t *d_fb, int w, int h, int
     const uint32_t *fb = reinterpret_cast<const uint32_t *>(d_fb) + (long long)f0 * npix;
     char *base = ctx->sixel_work.as<char>();
     B2_KERNEL(ctx, "sixel_palette_kernel");
-    {
-        const size_t t_words = W.ent_cap > 16384 ? (size_t)W.ent_cap : 16384;
-        const size_t smem_tables = sizeof(uint32_t) * (t_words + (size_t)W.ent_cap);
-        if (smem_tables <= 200 * 1024) sixel_palette_kernel<true, PaletteUniform><<<n, PT, smem_tables, ctx->stream>>>(fb, w, h, W, NoMixed());
-        else sixel_palette_kernel<false, PaletteUniform><<<n, PT, 65536, ctx->stream>>>(fb, w, h, W, NoMixed());
-    }
+    if (S.pal.smem_tables) sixel_palette_kernel<true, PaletteUniform><<<n, PT, S.pal.tables_smem, ctx->stream>>>(fb, w, h, W, NoMixed());
+    else sixel_palette_kernel<false, PaletteUniform><<<n, PT, 65536, ctx->stream>>>(fb, w, h, W, NoMixed());
     B2_LAUNCH_CHECK(ctx);
     B2_KERNEL(ctx, "sixel_lut_kernel");
     sixel_lut_kernel<<<dim3(128, n), 256, 0, ctx->stream>>>(W);
@@ -1416,9 +1437,9 @@ int plan_sixel_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *mb, MixedPla
         MixedSixelFrame &D = desc[f];
         const int w = F.out_w, h = (F.out_h + 5) / 6 * 6;
         const long long npix = (long long)w * h;
-        long long step_px = npix / 18383; if (npix < 18383) step_px = 6; if (step_px == 0) step_px = 1;   // as sixel_plan
+        const SixelPaletteShape P = sixel_palette_shape(npix);
         D.w = w; D.h = h;
-        D.ent_cap = (int)std::min<long long>(32768, (npix + step_px - 1) / step_px);
+        D.ent_cap = P.ent_cap;
         D.nb32 = (h + 31) / 32; D.nbands = h / 6;
         D.fb_px = px; px += (unsigned long long)npix;
         D.idx = idx; idx += align_up((size_t)npix, 16);
@@ -1429,14 +1450,12 @@ int plan_sixel_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *mb, MixedPla
         D.scr = scr; scr += D.band_cap * D.nbands;
         D.band0 = (int)bands; band_start[f] = bands; bands += (unsigned)D.nbands;
         D.cols_per_warp = ((w + EW - 1) / EW + 31) / 32 * 32;
-        int fw = 1;
-        const int per_frame = sixel_dither_split(D.nb32, n, ctx->sm_count, &D.bands_per_cta, &fw);
-        nwarps = std::max(nwarps, fw);
-        split |= per_frame > 1;
-        cta_start[f] = ctas; ctas += (unsigned)per_frame;
-        const size_t t_words = D.ent_cap > 16384 ? (size_t)D.ent_cap : 16384;
-        const size_t smem_tables = sizeof(uint32_t) * (t_words + (size_t)D.ent_cap);
-        if (smem_tables <= 200 * 1024) { list[0].push_back(f); pal_smem = std::max(pal_smem, smem_tables); }
+        const SixelDitherShape DS = sixel_dither_shape(D.nb32, n, n, ctx->sm_count, false);
+        D.bands_per_cta = DS.bands_per_cta;
+        nwarps = std::max(nwarps, DS.nwarps);
+        split |= DS.per_frame > 1;
+        cta_start[f] = ctas; ctas += (unsigned)DS.per_frame;
+        if (P.smem_tables) { list[0].push_back(f); pal_smem = std::max(pal_smem, P.tables_smem); }
         else list[1].push_back(f);
         wmax = std::max(wmax, w);
     }
@@ -1520,6 +1539,22 @@ int sixel_debug_fetch(b200timg_ctx *ctx, uint32_t *h_palette, uint32_t *h_counts
 }
 
 }  // namespace b200timg
+
+extern "C" int b200timg_sixel_shape_of(int w, int h, int n_frames, int n_total, int sm_count, b200timg_sixel_shape *out) {
+    using namespace b200timg;
+    char why[96];
+    if (!out || sm_count <= 0 || n_frames <= 0 || n_total < n_frames) return B200TIMG_EINVAL;
+    if (sixel_check_geometry(w, h, n_total, why, sizeof why) != B200TIMG_OK) return B200TIMG_EINVAL;      // as sixel_plan
+    const SixelPaletteShape P = sixel_palette_shape((long long)w * h);
+    out->step_px = (int)P.step_px; out->ent_cap = P.ent_cap; out->palette_global = P.smem_tables ? 0 : 1;
+    out->nb32 = (h + 31) / 32;
+    const SixelDitherShape D = sixel_dither_shape(out->nb32, n_frames, n_total, sm_count, true);
+    out->dither_ctas = D.per_frame; out->bands_per_cta = D.bands_per_cta; out->dither_warps = D.nwarps; out->dither_rounds = D.rounds;
+    out->emit_mode = sixel_emit_mode(w);
+    int cpw;
+    sixel_emit_tiling(w, &out->emit_tiles, &out->tile_w, &cpw);
+    return B200TIMG_OK;
+}
 
 #ifdef B200TIMG_EMIT_CLOCKS
 // instrumented builds only: the summed phase clocks [2][8] since the last call (then cleared); 0 or -3 (CUDA error)

@@ -120,7 +120,27 @@ int launch_sixel_emit3(b200timg_ctx *ctx, int w, int h, int n_frames, const Sixe
                        uint64_t *d_offsets);
 size_t sixel_dither_workspace(int w, int h, int n_frames, size_t *o_bnd, size_t *o_prog);
 int launch_sixel_dither(b200timg_ctx *ctx, const uint32_t *fb, int w, int h, int n_frames, int n_total, const SixelWork &W, void *d_bnd, void *d_prog);
-int sixel_dither_split(int nb32, int n_frames, int sm_count, int *bands_per_cta, int *nwarps);
+
+// ---- launch shapes (host).  The launchers and b200timg_sixel_shape_of both call these, so what the introspection reports
+// is what a launch does.
+// What the sixel path takes: h a multiple of 6, w <= 99999, h <= 65536 (2048 bands of 32 rows), n_frames <= 65535 and at
+// most 2^31 - 1 emit CTAs.  B200TIMG_OK, or B200TIMG_EINVAL with the reason in msg.
+int sixel_check_geometry(int w, int h, int n_frames, char *msg, size_t msg_cap);
+// K4 of a frame of npix pixels: sampling step, entries of each median-cut table, and whether the two tables fit the
+// palette kernel's shared memory (tables_smem bytes) or live in global memory.
+struct SixelPaletteShape { long long step_px; int ent_cap; bool smem_tables; size_t tables_smem; };
+SixelPaletteShape sixel_palette_shape(long long npix);
+// K5 of a launch over n_frames frames of nb32 bands, a slice of a batch of n_total: CTAs per frame, bands per CTA, warps
+// per CTA and rounds of a warp over its CTA's bands.  A frame is split only when the batch has fewer frames than SMs, and
+// then into at most sm_count / n_frames CTAs, so that every CTA of the launch is resident at once (bands wait for the
+// band above).  env: honour B200TIMG_DITHER_SPLIT / B200TIMG_DITHER_WARPS (the uniform launches do, mixed batches do not).
+struct SixelDitherShape { int per_frame, bands_per_cta, nwarps, rounds; };
+SixelDitherShape sixel_dither_shape(int nb32, int n_frames, int n_total, int sm_count, bool env);
+// K6: the emitter a frame w wide takes (1 v1, 4 v1b, 5 emit5: band scratch + compaction; 2 emit2, 3 emit3: single pass;
+// B200TIMG_EMIT / B200TIMG_EMIT_V2 honoured) and the single-pass emitters' column tiles.
+int sixel_emit_mode(int w);
+void sixel_emit_tiling(int w, int *ntiles, int *tw, int *cpw);
+
 int launch_sixel_dither_mixed(b200timg_ctx *ctx, const uint32_t *fb, unsigned n_ctas, const MixedSixelParams &M, const SixelWork &W,
                               void *d_bnd, void *d_prog, size_t n_prog, bool split);
 size_t sixel_emit_workspace(int w, int h, int n_frames, size_t *o_hdr_bytes, size_t *o_desc, size_t *o_ctl);

@@ -294,6 +294,27 @@ size_t sixel_dither_workspace(int w, int h, int n_frames, size_t *o_bnd, size_t 
     return off;
 }
 
+SixelDitherShape sixel_dither_shape(int nb32, int n_frames, int n_total, int sm_count, bool env) {
+    SixelDitherShape S;
+    // CTAs per frame: 1 when the batch fills the GPU, more (up to one round of bands per CTA) for small batches.
+    // All CTAs of a launch must be resident together when a frame is split (bands wait for the band above).
+    int per_frame = 1;
+    if (n_total < sm_count) {
+        per_frame = std::max(1, std::min(sm_count / n_total, (nb32 + 7) / 8));
+        if (const char *e = env ? getenv("B200TIMG_DITHER_SPLIT") : nullptr) per_frame = std::max(1, std::min(atoi(e), nb32));
+        if ((long long)per_frame * n_frames > sm_count) per_frame = std::max(1, sm_count / n_frames);
+    }
+    S.bands_per_cta = (nb32 + per_frame - 1) / per_frame;
+    S.per_frame = (nb32 + S.bands_per_cta - 1) / S.bands_per_cta;
+    // warps per CTA: full rounds over the CTA's bands.  Fewer warps = more rounds but a smaller share of the time spent
+    // filling and draining the band pipeline (each band starts ~80 columns behind the one above).
+    int wmax = D2_WMAX;
+    if (const char *e = env ? getenv("B200TIMG_DITHER_WARPS") : nullptr) wmax = std::max(1, std::min(atoi(e), D2_WMAX));
+    S.rounds = (S.bands_per_cta + wmax - 1) / wmax;
+    S.nwarps = (S.bands_per_cta + S.rounds - 1) / S.rounds;
+    return S;
+}
+
 // n_frames: frames of this launch (fb, W, d_bnd and d_prog already point at its first frame); n_total: frames of the
 // whole batch this launch is a slice of -- the "split a frame over several CTAs" decision looks at the batch, so a
 // slice that shares the GPU with another slice does not spread itself over every SM.
@@ -304,23 +325,10 @@ int launch_sixel_dither(b200timg_ctx *ctx, const uint32_t *fb, int w, int h, int
     // noticeable share of the kernel's issue slots in the wait loop, slots the producing warps need.
     G.spin_ns = 256;
     if (const char *e = getenv("B200TIMG_DITHER_SPIN")) G.spin_ns = (unsigned)std::max(0, std::min(atoi(e), 100000));
-    // CTAs per frame: 1 when the batch fills the GPU, more (up to one round of bands per CTA) for small batches.
-    // All CTAs of a launch must be resident together when a frame is split (bands wait for the band above).
-    int per_frame = 1;
-    if (n_total < ctx->sm_count) {
-        per_frame = std::max(1, std::min(ctx->sm_count / n_total, (G.nb32 + 7) / 8));
-        if (const char *e = getenv("B200TIMG_DITHER_SPLIT")) per_frame = std::max(1, std::min(atoi(e), G.nb32));
-        if ((long long)per_frame * n_frames > ctx->sm_count) per_frame = std::max(1, ctx->sm_count / n_frames);
-    }
-    G.bands_per_cta = (G.nb32 + per_frame - 1) / per_frame;
-    per_frame = (G.nb32 + G.bands_per_cta - 1) / G.bands_per_cta;
-    // warps per CTA: full rounds over the CTA's bands.  Fewer warps = more rounds but a smaller share of the time spent
-    // filling and draining the band pipeline (each band starts ~80 columns behind the one above).
-    int wmax = D2_WMAX;
-    if (const char *e = getenv("B200TIMG_DITHER_WARPS")) wmax = std::max(1, std::min(atoi(e), D2_WMAX));
-    const int rounds = (G.bands_per_cta + wmax - 1) / wmax;
-    G.nwarps = (G.bands_per_cta + rounds - 1) / rounds;
-    if (G.bands_per_cta > 2048) return ctx->fail(B200TIMG_EINVAL, "sixel: frame too tall");
+    const SixelDitherShape S = sixel_dither_shape(G.nb32, n_frames, n_total, ctx->sm_count, true);
+    const int per_frame = S.per_frame;
+    G.bands_per_cta = S.bands_per_cta;
+    G.nwarps = S.nwarps;
     const size_t smem = 32768 + (size_t)G.nwarps * D2_WARP_SMEM;
     B2_CUDA(ctx, cudaFuncSetAttribute(sixel_dither2_kernel<DitherUniform>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32768 + D2_WMAX * D2_WARP_SMEM));
     if (per_frame > 1) B2_CUDA(ctx, cudaMemsetAsync(d_prog, 0, sizeof(int) * (size_t)G.nb32 * n_frames, ctx->stream));
@@ -328,18 +336,6 @@ int launch_sixel_dither(b200timg_ctx *ctx, const uint32_t *fb, int w, int h, int
     sixel_dither2_kernel<DitherUniform><<<dim3(per_frame, n_frames), G.nwarps * 32, smem, ctx->stream>>>(fb, G, W, static_cast<uint4 *>(d_bnd), static_cast<int *>(d_prog));
     B2_LAUNCH_CHECK(ctx);
     return B200TIMG_OK;
-}
-
-// Mixed batches: launch_sixel_dither's default split for one frame of nb32 bands in a batch of n_frames.  A frame is split
-// only when the batch has fewer frames than SMs, and then into at most sm_count / n_frames CTAs, so that every CTA of the
-// launch can be resident at once.  Returns the frame's CTAs; *bands_per_cta and *nwarps (the warps it would run with).
-int sixel_dither_split(int nb32, int n_frames, int sm_count, int *bands_per_cta, int *nwarps) {
-    int per_frame = 1;
-    if (n_frames < sm_count) per_frame = std::max(1, std::min(sm_count / n_frames, (nb32 + 7) / 8));
-    *bands_per_cta = (nb32 + per_frame - 1) / per_frame;
-    const int rounds = (*bands_per_cta + D2_WMAX - 1) / D2_WMAX;
-    *nwarps = (*bands_per_cta + rounds - 1) / rounds;
-    return (nb32 + *bands_per_cta - 1) / *bands_per_cta;
 }
 
 // One launch over every frame's dither CTAs (M.cta_start); the block size is the largest any frame asks for.
