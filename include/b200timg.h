@@ -289,8 +289,8 @@ int b200timg_blocks_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *b, cons
  * rows, the background composed into the pad strip only (SixelCanvas::Send), palette, Floyd-Steinberg dither, DCS
  * stream -- whatever the frame's place in the batch, the batch size or the variant called.  x_indent_cells and the
  * block flags are ignored (the cursor move is the caller's prefix, as for the uniform sixel batch);
- * B200TIMG_FAST_SCALE is accepted and ignored.  The default kernels always run (B200TIMG_EMIT, B200TIMG_DITHER_V1 and
- * B200TIMG_PARTS do not apply).  Rejected with B200TIMG_EINVAL besides the cases above: out_w > 4095 and a padded
+ * B200TIMG_FAST_SCALE is accepted and ignored.  The default kernels always run (B200TIMG_EMIT and B200TIMG_PARTS do
+ * not apply).  Rejected with B200TIMG_EINVAL besides the cases above: out_w > 4095 and a padded
  * height over 65536 rows (the message names the frame; wider images go through the uniform batch).
  * The _dev variant follows the OUTPUT CAPACITY CONTRACT above.  The host variant stages into the sum of
  * b200timg_sixel_bound(out_w, round_to_sixel(out_h)) over the frames and returns B200TIMG_ENOSPC with offsets[]

@@ -64,6 +64,7 @@ def lib():
         _sig(L, "orc_sixel_encode", C.c_long, [u8p, C.c_int, C.c_int, C.c_int, C.c_char_p, C.c_long, u8p,
                                               C.POINTER(C.c_int), C.POINTER(C.c_int), u8p])
         _sig(L, "orc_sixel_palette", C.c_int, [u8p, C.c_int, C.c_int, C.c_int, u8p, C.POINTER(C.c_int)])
+        _sig(L, "orc_sixel_stream", C.c_long, [u8p, C.c_int, C.c_int, u8p, C.c_int, C.c_char_p, C.c_long])
         _sig(L, "orc_sixel_decode", C.c_int, [C.c_char_p, C.c_long, u8p, C.c_long, C.POINTER(C.c_int),
                                               C.POINTER(C.c_int), C.POINTER(C.c_int)])
         _ORC = L
@@ -182,6 +183,19 @@ def sixel_palette(fb, mode=0):
     oc = C.c_int()
     n = lib().orc_sixel_palette(_ptr(fb), w, h, mode, _ptr(pal), C.byref(oc))
     return pal[:n], oc.value
+
+
+def sixel_stream(palette, index):
+    """The device emitters' bytes for a palette ([n,3] uint8) and an index plane ([h,w] uint8): the same framing as
+    sixel_encode, bands written colour by colour (see orc_sixel_stream in oracle/sixel_oracle.c)."""
+    pal = np.ascontiguousarray(palette, dtype=np.uint8).reshape(-1, 3)
+    idx = np.ascontiguousarray(index, dtype=np.uint8)
+    h, w = idx.shape
+    cap = 4096 + 256 * 24 + ((h + 5) // 6) * (6 * w * 14 + 256 * 6)    # <= 6 runs a column, <= 14 bytes with its gap
+    buf = C.create_string_buffer(cap)
+    n = lib().orc_sixel_stream(_ptr(idx), w, h, _ptr(pal), len(pal), buf, cap)
+    assert n > 0, n
+    return buf.raw[:n]
 
 
 def sixel_decode(data, max_px=1 << 26):

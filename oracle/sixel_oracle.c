@@ -212,9 +212,7 @@ static int put_node(emit_t *e, int x, const node_t *np) {  /* sixel_put_node */
     return x;
 }
 
-static long encode_body(const uint8_t *index, int w, int h, const uint8_t *palette, int ncolors, char *out, long cap) {
-    emit_t E = { out, out + cap, 0, 0, -1, 0 };
-    emit_t *e = &E;
+static void put_header(emit_t *e, int w, int h, const uint8_t *palette, int ncolors) {
     e_putc(e, 033); e_putc(e, 'P'); e_putc(e, 'q');                        /* sixel_encode_header */
     e_putc(e, '"'); e_putnum(e, 1); e_putc(e, ';'); e_putnum(e, 1); e_putc(e, ';'); e_putnum(e, w); e_putc(e, ';'); e_putnum(e, h);
     for (int n = 0; n < ncolors; n++) {                                    /* output_rgb_palette_definition */
@@ -223,6 +221,12 @@ static long encode_body(const uint8_t *index, int w, int h, const uint8_t *palet
         e_putnum(e, (palette[n * 3 + 1] * 100 + 127) / 255); e_putc(e, ';');
         e_putnum(e, (palette[n * 3 + 2] * 100 + 127) / 255);
     }
+}
+
+static long encode_body(const uint8_t *index, int w, int h, const uint8_t *palette, int ncolors, char *out, long cap) {
+    emit_t E = { out, out + cap, 0, 0, -1, 0 };
+    emit_t *e = &E;
+    put_header(e, w, h, palette, ncolors);
     uint8_t *map = (uint8_t *)calloc((size_t)ncolors * w, 1);
     node_t *pool = (node_t *)malloc((size_t)(ncolors * (w / 2 + 2)) * sizeof(node_t));
     int i = 0;
@@ -277,6 +281,52 @@ static long encode_body(const uint8_t *index, int w, int h, const uint8_t *palet
     }
     e_putc(e, 033); e_putc(e, '\\');                                       /* sixel_encode_footer */
     free(map); free(pool);
+    return E.overflow ? -1 : (long)(E.p - out);
+}
+
+/* ---- the device's byte stream (timg_b200/csrc/sixel.cu, sixel_emit.cu) ----
+ * The same header, palette definitions and ST as encode_body; a band, though, is written colour by colour instead of
+ * in libsixel's node order.  Within each 6-row band, for every colour present, in ascending order: '$' (except before
+ * the band's first colour), "#c", then every run of that colour (consecutive columns with the same row bits) as its
+ * gap of blank columns since the colour's previous run (or since x = 0) followed by the run itself, each written as
+ * "!n" + character when longer than 3 and as repeated characters otherwise.  '-' goes between bands.
+ * index: w*h palette indices; palette: ncolors RGB triples.  Returns bytes written, or -1 if cap was too small. */
+static void put_rep(emit_t *e, int n, int ch) {
+    if (n > 3) { e_putc(e, '!'); e_putnum(e, n); e_putc(e, ch); }
+    else for (int k = 0; k < n; k++) e_putc(e, ch);
+}
+
+long orc_sixel_stream(const uint8_t *index, int w, int h, const uint8_t *palette, int ncolors, char *out, long cap) {
+    emit_t E = { out, out + cap, 0, 0, -1, 0 };
+    emit_t *e = &E;
+    put_header(e, w, h, palette, ncolors);
+    uint8_t *bits = (uint8_t *)malloc((size_t)256 * w);       /* [colour][x]: the band's rows of that colour */
+    for (int y0 = 0; y0 < h; y0 += 6) {
+        memset(bits, 0, (size_t)256 * w);
+        for (int r = 0; r < 6 && y0 + r < h; r++)
+            for (int x = 0; x < w; x++) bits[(size_t)index[(long)(y0 + r) * w + x] * w + x] |= (uint8_t)(1 << r);
+        if (y0 > 0) e_putc(e, '-');
+        int first = 1;
+        for (int c = 0; c < 256; c++) {
+            const uint8_t *m = bits + (size_t)c * w;
+            int end = 0;                                       /* one past the colour's previous run */
+            for (int x = 0; x < w;) {
+                if (!m[x]) { x++; continue; }
+                if (end == 0) {                                /* the colour's first run in this band */
+                    if (!first) e_putc(e, '$');
+                    e_putc(e, '#'); e_putnum(e, c);
+                    first = 0;
+                }
+                int x1 = x + 1;
+                while (x1 < w && m[x1] == m[x]) x1++;
+                put_rep(e, x - end, '?');
+                put_rep(e, x1 - x, '?' + m[x]);
+                end = x = x1;
+            }
+        }
+    }
+    free(bits);
+    e_putc(e, 033); e_putc(e, '\\');
     return E.overflow ? -1 : (long)(E.p - out);
 }
 

@@ -14,8 +14,7 @@ from timg_b200 import synth
 # cells (median cut + Floyd-Steinberg), False = at most 256 (table lookup per pixel), None = not asserted
 Case = namedtuple("Case", "group name kind w h seed n n_total env expect diffuse")
 
-KNOBS = ("B200TIMG_DITHER_SPLIT", "B200TIMG_DITHER_WARPS", "B200TIMG_DITHER_SPIN", "B200TIMG_DITHER_V1", "B200TIMG_PARTS",
-         "B200TIMG_EMIT", "B200TIMG_EMIT_V2", "B200TIMG_EMIT_MATCH")
+KNOBS = ("B200TIMG_DITHER_SPLIT", "B200TIMG_DITHER_WARPS", "B200TIMG_DITHER_SPIN", "B200TIMG_PARTS", "B200TIMG_EMIT")
 SM_COUNTS = (132, 114, 108)          # H100 SXM, H100 PCIe and a smaller part: the host-side coverage check walks the table for each
 
 PALETTE_CLASSES = ("step6", "step1_shared", "step1_global", "step1_global_saturated", "step2_shared", "step2_global", "step3plus")

@@ -90,7 +90,7 @@ def test_scale_cuda_planar_path(ctx):
             ctx.profile(False)
             want = oracle.stb_resize(img, ow, oh, fmt)
             assert (got == want).all(), (iw, ih, ow, oh, kind, fmt, int(np.abs(got.astype(int) - want).max()))
-            if "resample_planar_kernel" in rep or "resample_v3_exact_kernel" in rep:     # v3 = opaque tiles, planar = the rest
+            if "resample_planar_kernel" in rep:     # v3 = opaque tiles, planar = the rest
                 assert _vfirst_small_taps(iw, ih, ow, oh)
                 ran_planar += 1
     assert ran_planar >= 50 or os.environ.get("B200TIMG_NO_PLANAR"), ran_planar

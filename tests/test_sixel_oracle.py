@@ -24,6 +24,30 @@ def test_stream_grammar_and_roundtrip():
     assert data.count(b"-") == 36 // 6 - 1
 
 
+def test_device_stream_by_hand():
+    """oracle.sixel_stream, the statement of the device emitters' bytes, on a 5x12 frame written out by hand."""
+    pal = np.array([[0, 0, 0], [255, 0, 0], [0, 0, 255]], np.uint8)
+    idx = np.zeros((12, 5), np.uint8)
+    idx[:6, 1:3] = 1
+    idx[0, 4] = 2
+    idx[6:] = 2
+    want = (b'\x1bPq"1;1;5;12#0;2;0;0;0#1;2;100;0;0#2;2;0;0;100'
+            b"#0~??~}$#1?~~$#2!4?@"      # band 0: colour 0's runs (a bits change at x=4 starts one), gaps as '?'
+            b"-#2!5~\x1b\\")             # band 1: one run of the whole width
+    assert oracle.sixel_stream(pal, idx) == want
+
+
+def test_device_stream_decodes_to_the_index_plane():
+    rng = np.random.default_rng(5)
+    for w, h, n, runs in [(1, 6, 1, 1), (97, 36, 256, 1), (300, 18, 5, 9), (4095, 12, 40, 60), (23, 24, 2, 3)]:
+        pal = rng.integers(0, 256, (n, 3), dtype=np.uint8)
+        idx = rng.integers(0, n, (h, (w + runs - 1) // runs), dtype=np.uint8).repeat(runs, 1)[:, :w].copy()
+        data = oracle.sixel_stream(pal, idx)
+        img, _ = oracle.sixel_decode(data)
+        assert (img == pct(pal)[idx]).all(), (w, h, n)
+        assert data.count(b"-") == h // 6 - 1
+
+
 def test_few_colours_means_no_dither():
     fb = np.zeros((12, 40, 4), np.uint8)
     fb[..., 3] = 255

@@ -6,8 +6,9 @@
 // reference's cost model (resample_tables.cu).  Every * and + is a separate IEEE rounding
 // (__fmul_rn/__fadd_rn), like the reference's SSE2 code.
 //
-// v1 layout: one thread per output pixel, taps read straight from global memory (the
-// working set of a tile stays in L1/L2).  Algorithmic bytes: 4*iw*ih read + 4*ow*oh written.
+// Kernels: copies for unscaled frames; <= 8 taps per axis: the v3 kernel (FAST arithmetic, opaque tiles), the
+// planar kernel (vertical first, rows of 16 bytes) and the fixed-tap kernel (either order); longer filters: the two
+// 1-D passes of the twopass_* kernels.  Algorithmic bytes: 4*iw*ih read + 4*ow*oh written.
 #include <algorithm>
 #include <cstdlib>
 #include <map>
@@ -66,17 +67,6 @@ struct ResampleParams {
     ComposeSpec cs;              // fused AlphaComposeBackground (cs.active == 0: none)
 };
 
-struct Px7 { float c[7]; };
-
-__device__ __forceinline__ void decode7(uint32_t p, int bgra, float *d) {
-    const float k = 1.0f / 255.0f;
-    const float c0 = fmul((float)(p & 0xff), k), c1 = fmul((float)((p >> 8) & 0xff), k);
-    const float c2 = fmul((float)((p >> 16) & 0xff), k), a = fmul((float)(p >> 24), k);
-    const float r = bgra ? c2 : c0, b = bgra ? c0 : c2;
-    d[0] = r; d[1] = c1; d[2] = b; d[3] = a;
-    d[4] = fmul(r, a); d[5] = fmul(c1, a); d[6] = fmul(b, a);
-}
-
 __device__ __forceinline__ uint32_t encode_px(const float *e) {
     float r = e[0], g = e[1], b = e[2];
     const float a = e[3];
@@ -91,89 +81,6 @@ __device__ __forceinline__ uint32_t encode_px(const float *e) {
     };
     return pack_rgba(enc(r), enc(g), enc(b), enc(a));
 }
-
-template <bool VFIRST>
-__global__ void __launch_bounds__(256)
-resample_direct_kernel(const uint32_t *__restrict__ in, uint32_t *__restrict__ out, ResampleParams P) {
-    const int ox = blockIdx.x * 32 + (threadIdx.x & 31);
-    const int oy = blockIdx.y * 8 + (threadIdx.x >> 5);
-    const int f = blockIdx.z;
-    if (ox >= P.ow || oy >= P.oh) return;
-    const uint32_t *src = in + (long long)f * P.iw * P.ih;
-    const int hn0 = P.h_first[ox], hcnt = P.h_count[ox];
-    const int hpar = P.h_sequential ? 0 : (P.h_lead[ox] & 1);
-    const int hmask = P.h_sequential ? 0 : 1;
-    const int vn0 = P.v_first[oy], vcnt = P.v_count[oy];
-    const float *hc = P.h_coeff + (long long)ox * P.h_widest;
-    const float *vc = P.v_coeff + (long long)oy * P.v_widest;
-    float res[7];
-    if (!VFIRST) {
-        // rows: horizontal sum per input row, then accumulate rows in order
-        for (int k = 0; k < vcnt; ++k) {
-            const uint32_t *row = src + (long long)(vn0 + k) * P.iw + hn0;
-            float acc[2][7];
-#pragma unroll
-            for (int c = 0; c < 7; ++c) { acc[0][c] = 0.0f; acc[1][c] = 0.0f; }
-            for (int i = 0; i < hcnt; ++i) {
-                float d[7];
-                decode7(row[i], P.bgra, d);
-                const float w = hc[i];
-                const int p = (i + hpar) & hmask;
-#pragma unroll
-                for (int c = 0; c < 7; ++c) {
-                    const float t = fmul(d[c], w);
-                    if (p) acc[1][c] = fadd(acc[1][c], t); else acc[0][c] = fadd(acc[0][c], t);
-                }
-            }
-            const float wv = vc[k];
-#pragma unroll
-            for (int c = 0; c < 7; ++c) {
-                const float hsum = fadd(acc[0][c], acc[1][c]);
-                const float t = fmul(hsum, wv);
-                res[c] = (k == 0) ? t : fadd(res[c], t);
-            }
-        }
-    } else {
-        float acc[2][7];
-#pragma unroll
-        for (int c = 0; c < 7; ++c) { acc[0][c] = 0.0f; acc[1][c] = 0.0f; }
-        for (int i = 0; i < hcnt; ++i) {
-            const uint32_t *col = src + (long long)vn0 * P.iw + hn0 + i;
-            float vs[7];
-            for (int k = 0; k < vcnt; ++k) {
-                float d[7];
-                decode7(col[(long long)k * P.iw], P.bgra, d);
-                const float wv = vc[k];
-#pragma unroll
-                for (int c = 0; c < 7; ++c) {
-                    const float t = fmul(d[c], wv);
-                    vs[c] = (k == 0) ? t : fadd(vs[c], t);
-                }
-            }
-            const float w = hc[i];
-            const int p = (i + hpar) & hmask;
-#pragma unroll
-            for (int c = 0; c < 7; ++c) {
-                const float t = fmul(vs[c], w);
-                if (p) acc[1][c] = fadd(acc[1][c], t); else acc[0][c] = fadd(acc[0][c], t);
-            }
-        }
-#pragma unroll
-        for (int c = 0; c < 7; ++c) res[c] = fadd(acc[0][c], acc[1][c]);
-    }
-    out[((long long)f * P.out_frame_rows + oy) * P.ow + ox] = compose_at(P.cs, encode_px(res), ox, oy);
-}
-
-// ---- tiled separable kernel ---------------------------------------------------------------
-// One CTA produces a TW x TH output tile.  The input window the tile needs is decoded ONCE into
-// shared memory as float4 pixels, the first pass (vertical or horizontal, whichever the
-// reference's cost model picks) writes a float4 intermediate tile to shared memory, the second
-// pass reads it.  Arithmetic and summation order are exactly those of resample_direct_kernel;
-// only the sharing of partial sums between neighbouring output pixels is new.
-// Only 4 of the 7 channels are carried (A, R*A, G*A, B*A): the un-weighted R,G,B are needed only
-// where the filtered alpha is < 2^-120 (fully transparent output), and tiles that contain such a
-// pixel run a second pass for them.
-struct TileGeom { int tw, th, nix_max, niy_max; };
 
 // byte k of p as a float without the (quarter-rate) I2F unit: 0x4B0000bb is 2^23 + bb exactly.
 __device__ __forceinline__ float byte_f(uint32_t p, int k) {
@@ -200,156 +107,13 @@ __device__ __forceinline__ float4 decode_sel(uint32_t p, int bgra, bool plain) {
 __device__ __forceinline__ float4 mul4(float4 v, float w) { return make_float4(fmul(v.x, w), fmul(v.y, w), fmul(v.z, w), fmul(v.w, w)); }
 __device__ __forceinline__ float4 add4(float4 a, float4 b) { return make_float4(fadd(a.x, b.x), fadd(a.y, b.y), fadd(a.z, b.z), fadd(a.w, b.w)); }
 
-constexpr int RT = 256;      // threads per tile CTA
-constexpr int RPPT = 4;      // max output pixels per thread (TW*TH <= RT*RPPT)
-
-// Tap loops.  HW / VW > 0: compile-time tap budget (taps beyond an output's own count are skipped
-// by predicate, the loop is fully unrolled); 0: run-time loop.  Horizontal taps go alternately to
-// two accumulators and the two are added at the end -- which accumulator gets the even taps does
-// not matter because IEEE addition is commutative, so the reference's "leading zero taps" (which
-// only flip that assignment) need no special handling here.
-template <int VW>
-__device__ __forceinline__ float4 vsum(const float4 *col, int stride, int cnt, const float *vc) {
-    float4 a = mul4(col[0], vc[0]);
-    if (VW > 0) {
-#pragma unroll
-        for (int k = 1; k < VW; ++k) if (k < cnt) a = add4(a, mul4(col[k * stride], vc[k]));
-    } else {
-        for (int k = 1; k < cnt; ++k) a = add4(a, mul4(col[k * stride], vc[k]));
-    }
-    return a;
-}
-template <int HW>
-__device__ __forceinline__ float4 hsum(const float4 *row, int cnt, const float *hc, bool sequential) {
-    const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-    float4 a0 = z, a1 = z;
-    if (sequential) {
-        a0 = mul4(row[0], hc[0]);
-#pragma unroll
-        for (int i = 1; i < 3; ++i) if (i < cnt) a0 = add4(a0, mul4(row[i], hc[i]));
-        return a0;
-    }
-    if (HW > 0) {
-#pragma unroll
-        for (int i = 0; i < HW; ++i) if (i < cnt) { const float4 t = mul4(row[i], hc[i]); if (i & 1) a1 = add4(a1, t); else a0 = add4(a0, t); }
-    } else {
-        for (int i = 0; i < cnt; ++i) { const float4 t = mul4(row[i], hc[i]); if (i & 1) a1 = add4(a1, t); else a0 = add4(a0, t); }
-    }
-    return add4(a0, a1);
-}
-
-template <bool VFIRST, int HW, int VW>
-__global__ void __launch_bounds__(RT)
-resample_tiled_kernel(const uint32_t *__restrict__ in, uint32_t *__restrict__ out, ResampleParams P, TileGeom G) {
-    extern __shared__ float4 s_px[];                  // Din[niy][nix], T, then the tile's tap tables
-    __shared__ int s_ext[4];                          // ix0, ix1, iy0, iy1
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, f = blockIdx.z;
-    const int ox0 = blockIdx.x * G.tw, oy0 = blockIdx.y * G.th;
-    const int tw = min(G.tw, P.ow - ox0), th = min(G.th, P.oh - oy0);
-    const int dstride = G.nix_max;
-    float4 *Din = s_px;
-    float4 *T = s_px + (size_t)G.niy_max * dstride;
-    const int t_elems = VFIRST ? G.th * dstride : G.niy_max * G.tw;
-    int *s_hmeta = reinterpret_cast<int *>(T + t_elems);           // [tw][2] first, count
-    int *s_vmeta = s_hmeta + 2 * G.tw;                             // [th][2]
-    const int hstride = P.h_widest | 1, vstride = P.v_widest | 1;  // odd: conflict-free
-    float *s_hc = reinterpret_cast<float *>(s_vmeta + 2 * G.th);   // [tw][hstride]
-    float *s_vc = s_hc + G.tw * hstride;                           // [th][vstride]
-    if (tid == 0) { s_ext[0] = 0x7fffffff; s_ext[1] = -1; s_ext[2] = 0x7fffffff; s_ext[3] = -1; }
-    __syncthreads();
-    if (tid < tw) {
-        const int a = P.h_first[ox0 + tid], c = P.h_count[ox0 + tid];
-        s_hmeta[2 * tid] = a; s_hmeta[2 * tid + 1] = c;
-        atomicMin(&s_ext[0], a); atomicMax(&s_ext[1], a + c - 1);
-    }
-    if (tid >= 64 && tid - 64 < th) {
-        const int t = tid - 64, a = P.v_first[oy0 + t], c = P.v_count[oy0 + t];
-        s_vmeta[2 * t] = a; s_vmeta[2 * t + 1] = c;
-        atomicMin(&s_ext[2], a); atomicMax(&s_ext[3], a + c - 1);
-    }
-    for (int e = tid; e < tw * P.h_widest; e += RT) { const int x = e / P.h_widest, i = e - x * P.h_widest; s_hc[x * hstride + i] = P.h_coeff[(long long)(ox0 + x) * P.h_widest + i]; }
-    for (int e = tid; e < th * P.v_widest; e += RT) { const int y = e / P.v_widest, i = e - y * P.v_widest; s_vc[y * vstride + i] = P.v_coeff[(long long)(oy0 + y) * P.v_widest + i]; }
-    __syncthreads();
-    const int ix0 = s_ext[0], nix = s_ext[1] - ix0 + 1, iy0 = s_ext[2], niy = s_ext[3] - iy0 + 1;
-    const uint32_t *src = in + (long long)f * P.iw * P.ih;
-    const bool hseq = P.h_sequential != 0;
-    const float tiny = 7.5231638452626401e-37f;       // 2^-120
-    // this thread's output pixels: one column tx, rows ty0 + q*rstep (they share the horizontal taps)
-    const int tx = tid & (G.tw - 1), ty0 = tid / G.tw, rstep = RT / G.tw;
-    const bool col_ok = tx < tw;
-
-    float4 res[RPPT], plain[RPPT];
-    bool need_plain = false;
-    for (int pass = 0; pass < 2; ++pass) {
-        for (int ly = wid; ly < niy; ly += RT / 32) {            // stage + decode once; a warp per row
-            const uint32_t *row = src + (long long)(iy0 + ly) * P.iw + ix0;
-            float4 *drow = Din + ly * dstride;
-            for (int lx = lane; lx < nix; lx += 32) drow[lx] = pass == 0 ? decode_pm(row[lx], P.bgra) : decode_plain(row[lx], P.bgra);
-        }
-        __syncthreads();
-        float4 acc[RPPT];
-        if (VFIRST) {
-            for (int ty = wid; ty < th; ty += RT / 32) {         // T[ty][lx] = sum_k Din[v_first+k][lx]*cv[k], rows in order
-                const int n0 = s_vmeta[2 * ty] - iy0, cnt = s_vmeta[2 * ty + 1];
-                const float *vc = s_vc + ty * vstride;
-                const float4 *dcol = Din + n0 * dstride;
-                float4 *trow = T + ty * dstride;
-                for (int lx = lane; lx < nix; lx += 32) trow[lx] = vsum<VW>(dcol + lx, dstride, cnt, vc);
-            }
-            __syncthreads();
-            if (col_ok) {
-                const int n0 = s_hmeta[2 * tx] - ix0, cnt = s_hmeta[2 * tx + 1];
-                const float *hc = s_hc + tx * hstride;
-#pragma unroll
-                for (int q = 0; q < RPPT; ++q) {
-                    const int ty = ty0 + q * rstep;
-                    if (ty < th) acc[q] = hsum<HW>(T + ty * dstride + n0, cnt, hc, hseq);
-                }
-            }
-        } else {
-            if (col_ok) {                                        // T[ly][tx] = sum_i Din[ly][h_first+i]*ch[i]
-                const int n0 = s_hmeta[2 * tx] - ix0, cnt = s_hmeta[2 * tx + 1];
-                const float *hc = s_hc + tx * hstride;
-                for (int ly = ty0; ly < niy; ly += rstep) T[ly * G.tw + tx] = hsum<HW>(Din + ly * dstride + n0, cnt, hc, hseq);
-            }
-            __syncthreads();
-            if (col_ok) {
-#pragma unroll
-                for (int q = 0; q < RPPT; ++q) {
-                    const int ty = ty0 + q * rstep;
-                    if (ty < th) {
-                        const int n0 = s_vmeta[2 * ty] - iy0, cnt = s_vmeta[2 * ty + 1];
-                        acc[q] = vsum<VW>(T + n0 * G.tw + tx, G.tw, cnt, s_vc + ty * vstride);
-                    }
-                }
-            }
-        }
-#pragma unroll
-        for (int q = 0; q < RPPT; ++q) { if (pass == 0) res[q] = acc[q]; else plain[q] = acc[q]; }
-        if (pass == 0) {
-#pragma unroll
-            for (int q = 0; q < RPPT; ++q) if (col_ok && ty0 + q * rstep < th && res[q].w < tiny) need_plain = true;
-            if (!__syncthreads_or(need_plain)) break;          // also orders T/Din reuse for pass 1
-        }
-    }
-    if (col_ok) {
-#pragma unroll
-        for (int q = 0; q < RPPT; ++q) {
-            const int ty = ty0 + q * rstep;
-            if (ty < th) {
-                float v[7];
-                v[3] = res[q].w; v[4] = res[q].x; v[5] = res[q].y; v[6] = res[q].z;
-                const bool transparent = res[q].w < tiny;
-                v[0] = transparent ? plain[q].x : 0.f; v[1] = transparent ? plain[q].y : 0.f; v[2] = transparent ? plain[q].z : 0.f;
-                out[((long long)f * P.out_frame_rows + oy0 + ty) * P.ow + ox0 + tx] = compose_at(P.cs, encode_px(v), ox0 + tx, oy0 + ty);
-            }
-        }
-    }
-}
-
 // ---- fixed-tap fast path ------------------------------------------------------------------
-// Same algorithm as resample_tiled_kernel, specialised so the inner loops carry no predicates and
-// no run-time trip counts: every output uses exactly HC horizontal and VC vertical taps (the
+// One CTA produces a tile of output pixels.  The input window the tile needs is decoded ONCE into shared memory as
+// float4 pixels, the first pass (vertical or horizontal, whichever the reference's cost model picks) writes a float4
+// intermediate tile to shared memory, the second pass reads it.  Only 4 of the 7 channels are carried (A, R*A, G*A,
+// B*A): the un-weighted R,G,B are needed only where the filtered alpha is < 2^-120 (fully transparent output), and
+// tiles that contain such a pixel run a second pass for them.  The kernel is specialised so the inner loops carry no
+// predicates and no run-time trip counts: every output uses exactly HC horizontal and VC vertical taps (the
 // per-axis widest count rounded up to 2/4/6/8); taps an output does not have are zero coefficients
 // reading staged (finite) pixels, which adds +0 and changes nothing.  The staged window is padded
 // accordingly (zeros outside the image), its origin per tile column/row comes from the host.
@@ -793,7 +557,7 @@ struct FixedVariant { FixedFn fn; int th, nt; };
 // Tile 64x16, 256 threads, 3 CTAs/SM (80 registers of the SM's 64 K), chosen among {16x256x3, 16x256x4,
 // 8x128x8, 8x256x4, 16x512x2, 32x512x2} for C2 frames.
 template <bool VF, int HC>
-static FixedVariant fixed_v(int vc, char v) {
+static FixedVariant fixed_v(int vc) {
     switch (vc) {
     case 2: return {resample_fixed_kernel<VF, HC, 2, 16, 256, 3>, 16, 256};
     case 4: return {resample_fixed_kernel<VF, HC, 4, 16, 256, 3>, 16, 256};
@@ -802,47 +566,26 @@ static FixedVariant fixed_v(int vc, char v) {
     }
 }
 template <bool VF>
-static FixedVariant fixed_h(int hc, int vc, char v) {
+static FixedVariant fixed_h(int hc, int vc) {
     switch (hc) {
-    case 2: return fixed_v<VF, 2>(vc, v);
-    case 4: return fixed_v<VF, 4>(vc, v);
-    case 6: return fixed_v<VF, 6>(vc, v);
-    default: return fixed_v<VF, 8>(vc, v);
+    case 2: return fixed_v<VF, 2>(vc);
+    case 4: return fixed_v<VF, 4>(vc);
+    case 6: return fixed_v<VF, 6>(vc);
+    default: return fixed_v<VF, 8>(vc);
     }
 }
 static int fixed_class(int widest) { return widest <= 2 ? 2 : widest <= 4 ? 4 : widest <= 6 ? 6 : 8; }
 
-typedef void (*TiledFn)(const uint32_t *, uint32_t *, ResampleParams, TileGeom);
-template <bool VF, int HW>
-static TiledFn pick_v(int vclass) {
-    switch (vclass) {
-    case 4: return resample_tiled_kernel<VF, HW, 4>;
-    case 6: return resample_tiled_kernel<VF, HW, 6>;
-    case 8: return resample_tiled_kernel<VF, HW, 8>;
-    default: return resample_tiled_kernel<VF, HW, 0>;
-    }
-}
-template <bool VF>
-static TiledFn pick_h(int hclass, int vclass) {
-    switch (hclass) {
-    case 4: return pick_v<VF, 4>(vclass);
-    case 6: return pick_v<VF, 6>(vclass);
-    case 8: return pick_v<VF, 8>(vclass);
-    default: return pick_v<VF, 0>(vclass);
-    }
-}
-static int tap_class(int widest) { return widest <= 4 ? 4 : widest <= 6 ? 6 : widest <= 8 ? 8 : 0; }
-
 
 // ---- two-pass kernels for long filters (> 8 taps on an axis: strong downscales such as 4K -> a grid cell,
 // 1080p -> 160 columns) -----------------------------------------------------------------------------
-// The tiled kernel above stages a whole 2-D window per tile; with 24..48 taps per axis the window no longer
+// The fixed-tap kernels above stage a whole 2-D window per tile; with 24..48 taps per axis the window no longer
 // fits and its halo dwarfs the tile.  Here each pass is a plain 1-D filter over a float4 intermediate image
 // (R*A, G*A, B*A, A) kept in global memory (a few MB per frame, written and read once):
 //   pass 1 (the axis the reference's cost model runs first) decodes the source bytes on the fly,
 //   pass 2 filters the intermediate, un-weights, encodes, composes.
-// Same arithmetic and summation order as resample_direct_kernel (vertical taps in row order; horizontal taps
-// alternating between two accumulators, or sequential when <= 3).  Output pixels whose filtered alpha is below
+// The reference's arithmetic and summation order (vertical taps in row order; horizontal taps alternating between two
+// accumulators, or sequential when <= 3).  Output pixels whose filtered alpha is below
 // 2^-120 need the un-weighted colour planes: pass 2 raises a per-frame flag for them and a second pair of
 // passes (which return at once when the flag is down -- always, for opaque sources) fills them in.
 struct TwoPassParams {
@@ -1053,46 +796,26 @@ resample_copy4_kernel(const uint32_t *__restrict__ in, uint32_t *__restrict__ ou
 // v3 keeps the window as the RAW pixels (4 B/px: a plain 16-byte copy, no decode at staging) and turns
 // bytes into floats at the point of use (PRMT into the mantissa of 2^23, one FSUB), two neighbouring
 // columns per thread; the tap sums work on register PAIRS -- (R,G) of a pixel, (B,B) of two pixels.
-// Two arithmetic modes:
-//   EXACT  the reference's arithmetic bit for bit (byte * (1/255), every product and sum rounded
-//          separately: FMUL + FADD, never contracted), even/odd horizontal accumulators, analytic alpha
-//          of the all-opaque window, un-weight by 1/alpha, trunc(clamp(v * 255 + 0.5));
-//   FAST   the same filter with FFMA and the 1/255 .. *255 round trip dropped: within 1 LSB of the
-//          reference (BASELINE.md's stated gate for the Mitchell path); used where the result feeds the
-//          sixel quantiser, whose own parity is a delta-E tolerance.
+// The arithmetic is the FAST mode: the reference's filter with FFMA and the 1/255 .. *255 round trip dropped,
+// within 1 LSB of the reference (BASELINE.md's stated gate for the Mitchell path); used where the result feeds the
+// sixel quantiser, whose own parity is a delta-E tolerance.  (Bit-exact scaling takes the planar kernel.)
 // Tiles whose window is not fully opaque are handed to the planar kernel through a work list.
 struct F2 { float x, y; };
 #ifdef CUSIM
 __device__ __forceinline__ F2 f2_add(F2 a, F2 b) { return F2{a.x + b.x, a.y + b.y}; }
 __device__ __forceinline__ F2 f2_fma(F2 a, F2 b, F2 c) { return F2{fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)}; }
 #else
-// sm_90 has no packed FP32 arithmetic: each lane is one round-to-nearest FADD / FFMA (__fadd_rn is never
-// contracted with the product before it, which the EXACT mode relies on).
+// sm_90 has no packed FP32 arithmetic: each lane is one round-to-nearest FADD / FFMA.
 __device__ __forceinline__ F2 f2_add(F2 a, F2 b) { return F2{__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)}; }
 __device__ __forceinline__ F2 f2_fma(F2 a, F2 b, F2 c) { return F2{__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)}; }
 #endif
-// acc = v * c   /   acc += v * c   in the mode's arithmetic
-template <bool EXACT> __device__ __forceinline__ F2 f2_mul(F2 v, float c) {
-    if (EXACT) return F2{fmul(v.x, c), fmul(v.y, c)};
-    return f2_fma(v, F2{c, c}, F2{0.0f, 0.0f});
-}
-template <bool EXACT> __device__ __forceinline__ F2 f2_mac(F2 a, F2 v, float c) {
-    if (EXACT) return f2_add(a, F2{fmul(v.x, c), fmul(v.y, c)});
-    return f2_fma(v, F2{c, c}, a);
-}
-template <bool EXACT> __device__ __forceinline__ float f1_mac(float a, float v, float c) {
-    if (EXACT) return fadd(a, fmul(v, c));
-    return fmaf(v, c, a);
-}
-// byte `sel & 7` of p as a float: exact integer (FAST) or the reference's byte * (1/255) (EXACT)
-template <bool EXACT> __device__ __forceinline__ float byte_val(uint32_t p, uint32_t sel) {
-    const float v = fsub(__uint_as_float(__byte_perm(p, 0x4B000000u, sel)), 8388608.0f);
-    return EXACT ? fmul(v, 1.0f / 255.0f) : v;
-}
+// acc = v * c   /   acc += v * c
+__device__ __forceinline__ F2 f2_mul(F2 v, float c) { return f2_fma(v, F2{c, c}, F2{0.0f, 0.0f}); }
+__device__ __forceinline__ F2 f2_mac(F2 a, F2 v, float c) { return f2_fma(v, F2{c, c}, a); }
+__device__ __forceinline__ float f1_mac(float a, float v, float c) { return fmaf(v, c, a); }
 
-// two bytes -> a float pair.  FAST: two PRMTs into the mantissa of 2^23 and ONE packed subtraction.
-template <bool EXACT> __device__ __forceinline__ F2 byte_pair(uint32_t pa, uint32_t sa, uint32_t pb, uint32_t sb) {
-    if (EXACT) return F2{byte_val<true>(pa, sa), byte_val<true>(pb, sb)};
+// two bytes -> a float pair (exact integers): two PRMTs into the mantissa of 2^23 and ONE packed subtraction.
+__device__ __forceinline__ F2 byte_pair(uint32_t pa, uint32_t sa, uint32_t pb, uint32_t sb) {
     return f2_add(F2{__uint_as_float(__byte_perm(pa, 0x4B000000u, sa)), __uint_as_float(__byte_perm(pb, 0x4B000000u, sb))},
                   F2{-8388608.0f, -8388608.0f});
 }
@@ -1108,20 +831,14 @@ __device__ __forceinline__ uint32_t sat_u8(float v) {
 }
 
 struct V3Geom { int nix, niy, sp, tp; unsigned grp_magic; const int32_t *tile_ix0, *tile_iy0; uint32_t *fallback; int use_tma; };   // grp_magic: floor(2^32/(sp/4))+1
-// Tuning switches (tools/build_variant.sh builds variant libraries to compare on C2 frames):
-//   V3_SENT 0, 2 CTAs/SM asked (3 resident when it fits 80 registers)   <- default
-//   V3_SENT 1, 3 CTAs/SM forced (fewer registers, more instructions)
-//   V3_SENT 1, 2 CTAs/SM (more than 80 registers: only 2 resident)
-//   V3_SENT 0, 3 CTAs/SM forced (80 registers, spills)
-#ifndef V3_SENT
-#define V3_SENT 0            // 1: sentinel-terminated completion walks (no bound test), 0: bounded walks
-#endif
+// Tuning switch (tools/build_variant.sh builds variant libraries to compare on C2 frames): CTAs/SM asked of the
+// compiler.  2 (the default) leaves 3 resident when the kernel fits 80 registers; 3 forces 80 registers and spills.
 #ifndef V3_MINB_VALUE
 #define V3_MINB_VALUE 2
 #endif
 constexpr int V3_TW = 64, V3_TH = 32, V3_NT = 256, V3_MINB = V3_MINB_VALUE;   // 3 CTAs/SM: <= 80 registers (84 cost a third of the occupancy)
 
-template <int HC, int VC, bool EXACT>
+template <int HC, int VC>
 __global__ void __launch_bounds__(V3_NT, (VC >= 8 ? 2 : V3_MINB))      // the 8-row register windows do not fit 80 registers
 resample_v3_kernel(const uint32_t *__restrict__ in, uint32_t *__restrict__ out, ResampleParams P, V3Geom G,
                    const __grid_constant__ CUtensorMap tmap) {
@@ -1227,29 +944,29 @@ resample_v3_kernel(const uint32_t *__restrict__ in, uint32_t *__restrict__ out, 
                     if (r < rend) {
                         const uint2 pp = *reinterpret_cast<const uint2 *>(scol + r * sp);
                         amask &= pp.x & pp.y;
-                        w0[sl] = byte_pair<EXACT>(pp.x, sel_r, pp.x, sel_g);
-                        w1[sl] = byte_pair<EXACT>(pp.y, sel_r, pp.y, sel_g);
-                        wb[sl] = byte_pair<EXACT>(pp.x, sel_b, pp.y, sel_b);
+                        w0[sl] = byte_pair(pp.x, sel_r, pp.x, sel_g);
+                        w1[sl] = byte_pair(pp.y, sel_r, pp.y, sel_g);
+                        wb[sl] = byte_pair(pp.x, sel_b, pp.y, sel_b);
                         // uniform: every thread walks the same rows.  No j < j1 test: a row of the NEXT group completing at this
                         // very input row (only when enlarging) has exactly this window as its taps -- the duplicate write
                         // stores the same values the owner stores; the sentinel ends the walk at the tile's last row.
-                        while ((V3_SENT || j < j1) && ej == r) {
+                        while (j < j1 && ej == r) {
                             const float4 v0 = *reinterpret_cast<const float4 *>(s_vc + j * 8), v1 = *reinterpret_cast<const float4 *>(s_vc + j * 8 + 4);
                             const float vc[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
-                            F2 a0 = f2_mul<EXACT>(w0[(sl + 1) % VC], vc[0]), a1 = f2_mul<EXACT>(w1[(sl + 1) % VC], vc[0]);
-                            F2 ab = f2_mul<EXACT>(wb[(sl + 1) % VC], vc[0]);
+                            F2 a0 = f2_mul(w0[(sl + 1) % VC], vc[0]), a1 = f2_mul(w1[(sl + 1) % VC], vc[0]);
+                            F2 ab = f2_mul(wb[(sl + 1) % VC], vc[0]);
 #pragma unroll
                             for (int k = 1; k < VC; ++k) {
-                                a0 = f2_mac<EXACT>(a0, w0[(sl + 1 + k) % VC], vc[k]);
-                                a1 = f2_mac<EXACT>(a1, w1[(sl + 1 + k) % VC], vc[k]);
-                                ab = f2_mac<EXACT>(ab, wb[(sl + 1 + k) % VC], vc[k]);
+                                a0 = f2_mac(a0, w0[(sl + 1 + k) % VC], vc[k]);
+                                a1 = f2_mac(a1, w1[(sl + 1 + k) % VC], vc[k]);
+                                ab = f2_mac(ab, wb[(sl + 1 + k) % VC], vc[k]);
                             }
                             float2 *t = TRG + j * tp + 2 * cp;
                             t[0] = make_float2(a0.x, a0.y); t[1] = make_float2(a1.x, a1.y);
                             float *tb = TB + j * tp + 2 * cp;
                             tb[0] = ab.x; tb[1] = ab.y;
                             ++j;
-                            ej = (V3_SENT || j < j1) ? s_vlast[j] : -1;
+                            ej = j < j1 ? s_vlast[j] : -1;
                         }
                     }
                 }
@@ -1268,14 +985,6 @@ resample_v3_kernel(const uint32_t *__restrict__ in, uint32_t *__restrict__ out, 
     // and walks the intermediate columns they need once (window of HC columns in registers).  Pixels go straight
     // into the transpose buffer O (it aliases S, which is dead now).
     const bool hseq = P.h_sequential != 0;
-    float av = 0.0f;                                              // EXACT: vertical tap sum of an all-ones (alpha) column
-    if (EXACT) {
-        const float4 v0 = *reinterpret_cast<const float4 *>(s_vc + lane * 8), v1 = *reinterpret_cast<const float4 *>(s_vc + lane * 8 + 4);
-        const float vc[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
-        av = vc[0];
-#pragma unroll
-        for (int k = 1; k < VC; ++k) av = fadd(av, vc[k]);
-    }
     {
         const int tx0 = wid * 8, tx1 = tx0 + 8;
         const int f0 = s_hlast[tx0] - (HC - 1), cend = s_hlast[tx1 - 1] + 1;
@@ -1291,46 +1000,34 @@ resample_v3_kernel(const uint32_t *__restrict__ in, uint32_t *__restrict__ out, 
                 if (c < cend) {
                     const float2 q = trow[c];
                     wrg[sl] = F2{q.x, q.y}; wbb[sl] = brow[c];
-                    while ((V3_SENT || tx < tx1) && etx == c) {                // same argument as in the vertical walk
+                    while (tx < tx1 && etx == c) {                // same argument as in the vertical walk
                         const float4 h0 = *reinterpret_cast<const float4 *>(s_hc + tx * 8), h1 = *reinterpret_cast<const float4 *>(s_hc + tx * 8 + 4);
                         const float hc[8] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
-                        F2 c2; float cb, al = 1.0f;
+                        F2 c2; float cb;
                         if (hseq) {
-                            F2 a = f2_mul<EXACT>(wrg[(sl + 1) % HC], hc[0]);
-                            float b = EXACT ? fmul(wbb[(sl + 1) % HC], hc[0]) : wbb[(sl + 1) % HC] * hc[0];
-                            float aa = EXACT ? fmul(av, hc[0]) : 0.0f;
+                            F2 a = f2_mul(wrg[(sl + 1) % HC], hc[0]);
+                            float b = wbb[(sl + 1) % HC] * hc[0];
 #pragma unroll
                             for (int i = 1; i < (HC < 3 ? HC : 3); ++i) {
-                                a = f2_mac<EXACT>(a, wrg[(sl + 1 + i) % HC], hc[i]); b = f1_mac<EXACT>(b, wbb[(sl + 1 + i) % HC], hc[i]);
-                                if (EXACT) aa = fadd(aa, fmul(av, hc[i]));
+                                a = f2_mac(a, wrg[(sl + 1 + i) % HC], hc[i]); b = f1_mac(b, wbb[(sl + 1 + i) % HC], hc[i]);
                             }
-                            c2 = a; cb = b; if (EXACT) al = aa;
+                            c2 = a; cb = b;
                         } else {
-                            F2 a0 = f2_mul<EXACT>(wrg[(sl + 1) % HC], hc[0]), a1 = f2_mul<EXACT>(wrg[(sl + 2) % HC], hc[1]);
-                            float b0 = EXACT ? fmul(wbb[(sl + 1) % HC], hc[0]) : wbb[(sl + 1) % HC] * hc[0];
-                            float b1 = EXACT ? fmul(wbb[(sl + 2) % HC], hc[1]) : wbb[(sl + 2) % HC] * hc[1];
-                            float l0 = EXACT ? fmul(av, hc[0]) : 0.0f, l1 = EXACT ? fmul(av, hc[1]) : 0.0f;
+                            F2 a0 = f2_mul(wrg[(sl + 1) % HC], hc[0]), a1 = f2_mul(wrg[(sl + 2) % HC], hc[1]);
+                            float b0 = wbb[(sl + 1) % HC] * hc[0];
+                            float b1 = wbb[(sl + 2) % HC] * hc[1];
 #pragma unroll
                             for (int i = 2; i < HC; ++i) {
-                                if (i & 1) { a1 = f2_mac<EXACT>(a1, wrg[(sl + 1 + i) % HC], hc[i]); b1 = f1_mac<EXACT>(b1, wbb[(sl + 1 + i) % HC], hc[i]); if (EXACT) l1 = fadd(l1, fmul(av, hc[i])); }
-                                else { a0 = f2_mac<EXACT>(a0, wrg[(sl + 1 + i) % HC], hc[i]); b0 = f1_mac<EXACT>(b0, wbb[(sl + 1 + i) % HC], hc[i]); if (EXACT) l0 = fadd(l0, fmul(av, hc[i])); }
+                                if (i & 1) { a1 = f2_mac(a1, wrg[(sl + 1 + i) % HC], hc[i]); b1 = f1_mac(b1, wbb[(sl + 1 + i) % HC], hc[i]); }
+                                else { a0 = f2_mac(a0, wrg[(sl + 1 + i) % HC], hc[i]); b0 = f1_mac(b0, wbb[(sl + 1 + i) % HC], hc[i]); }
                             }
-                            c2 = EXACT ? f2_add(a0, a1) : F2{a0.x + a1.x, a0.y + a1.y};
-                            cb = EXACT ? fadd(b0, b1) : b0 + b1;
-                            if (EXACT) al = fadd(l0, l1);
+                            c2 = F2{a0.x + a1.x, a0.y + a1.y};
+                            cb = b0 + b1;
                         }
-                        uint32_t px;
-                        if (EXACT) {
-                            float v[7];
-                            v[0] = c2.x; v[1] = c2.y; v[2] = cb; v[3] = al; v[4] = c2.x; v[5] = c2.y; v[6] = cb;
-                            px = compose_at(P.cs, encode_px(v), ox0 + tx, oy0 + lane);
-                        } else {
-                            const uint32_t r8 = sat_u8(c2.x), g8 = sat_u8(c2.y), b8 = sat_u8(cb);
-                            px = pack_rgba(r8, g8, b8, 0xffu);                    // opaque in, opaque out: nothing to compose
-                        }
-                        O[lane * (V3_TW + 1) + tx] = px;
+                        const uint32_t r8 = sat_u8(c2.x), g8 = sat_u8(c2.y), b8 = sat_u8(cb);
+                        O[lane * (V3_TW + 1) + tx] = pack_rgba(r8, g8, b8, 0xffu);    // opaque in, opaque out: nothing to compose
                         ++tx;
-                        etx = (V3_SENT || tx < tx1) ? s_hlast[tx] : -1;
+                        etx = tx < tx1 ? s_hlast[tx] : -1;
                     }
                 }
             }
@@ -1377,22 +1074,21 @@ static bool v3_tensor_map(CUtensorMap *map, const uint32_t *src, int iw, int ih,
 }
 
 typedef void (*V3Fn)(const uint32_t *, uint32_t *, ResampleParams, V3Geom, const CUtensorMap);
-template <int HC, bool EXACT>
+template <int HC>
 static V3Fn v3_v(int vc) {
     switch (vc) {
-    case 2: return resample_v3_kernel<HC, 2, EXACT>;
-    case 4: return resample_v3_kernel<HC, 4, EXACT>;
-    case 6: return resample_v3_kernel<HC, 6, EXACT>;
-    default: return resample_v3_kernel<HC, 8, EXACT>;
+    case 2: return resample_v3_kernel<HC, 2>;
+    case 4: return resample_v3_kernel<HC, 4>;
+    case 6: return resample_v3_kernel<HC, 6>;
+    default: return resample_v3_kernel<HC, 8>;
     }
 }
-template <bool EXACT>
 static V3Fn v3_h(int hc, int vc) {
     switch (hc) {
-    case 2: return v3_v<2, EXACT>(vc);
-    case 4: return v3_v<4, EXACT>(vc);
-    case 6: return v3_v<6, EXACT>(vc);
-    default: return v3_v<8, EXACT>(vc);
+    case 2: return v3_v<2>(vc);
+    case 4: return v3_v<4>(vc);
+    case 6: return v3_v<6>(vc);
+    default: return v3_v<8>(vc);
     }
 }
 typedef void (*PlanarListFn)(const uint32_t *, uint32_t *, ResampleParams, PlanarGeom, const uint32_t *);
@@ -1486,7 +1182,7 @@ int launch_scale(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int fmt
         // fastest path: vertical pass first, <= 8 taps per axis, 16-byte aligned rows -> v3 kernel (opaque tiles)
         // with the planar kernel taking the tiles that contain transparency
         if (pl->vertical_first && pl->h.widest <= 8 && pl->v.widest <= 8 && (iw & 3) == 0 &&
-            (reinterpret_cast<uintptr_t>(d_in) & 15) == 0 && !getenv("B200TIMG_NO_PLANAR") && !getenv("B200TIMG_NO_FIXED")) {
+            (reinterpret_cast<uintptr_t>(d_in) & 15) == 0 && !getenv("B200TIMG_NO_PLANAR")) {
             const int hc = fixed_class(pl->h.widest), vc = fixed_class(pl->v.widest);
             auto tile_origins = [&](const AxisTable &T, int n_out, int tile, int taps, bool align4, std::vector<int32_t> &orig) -> int {
                 const int nt = (n_out + tile - 1) / tile;
@@ -1514,9 +1210,8 @@ int launch_scale(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int fmt
             const int sp3 = (nix3 + 3) & ~3, tp3 = sp3 | 1;
             const size_t v3smem = sizeof(uint32_t) * (size_t)niy * sp3 + (sizeof(float2) + sizeof(float)) * (size_t)V3_TH * tp3 + 16 +
                                   sizeof(float) * ((size_t)V3_TW * 8 + V3_TH * 8) + sizeof(int) * (V3_TW + V3_TH + 2);
-            // v3 pays off in the FAST arithmetic; in EXACT arithmetic its streaming passes are slower than the planar
-            // kernel, so bit-exact scaling stays on the planar kernel unless asked
-            const bool v3_ok = planar_ok && !getenv("B200TIMG_NO_V3") && (fast || getenv("B200TIMG_V3_EXACT")) && v3smem <= 100 * 1024 &&
+            // v3 pays off in the FAST arithmetic only; bit-exact scaling takes the planar kernel
+            const bool v3_ok = planar_ok && fast && v3smem <= 100 * 1024 &&
                                (size_t)V3_TH * (V3_TW + 1) <= (size_t)niy * sp3;
             if (planar_ok) {
                 B2_CUDA(ctx, ctx->misc.reserve(4096 + sizeof(int32_t) * (size_t)(ntx + nty + ntx3)));
@@ -1535,9 +1230,9 @@ int launch_scale(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int fmt
                     CUtensorMap tmap;
                     memset(&tmap, 0, sizeof tmap);
                     VG.use_tma = v3_tensor_map(&tmap, in, iw, ih, n_frames, sp3, niy) ? 1 : 0;
-                    V3Fn fn = fast ? v3_h<false>(hc, vc) : v3_h<true>(hc, vc);
+                    V3Fn fn = v3_h(hc, vc);
                     B2_CUDA(ctx, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-                    B2_KERNEL(ctx, fast ? "resample_v3_fast_kernel" : "resample_v3_exact_kernel");
+                    B2_KERNEL(ctx, "resample_v3_fast_kernel");
                     fn<<<dim3(ntx3, nty, n_frames), V3_NT, v3smem, ctx->stream>>>(in, out, P, VG, tmap);
                     B2_LAUNCH_CHECK(ctx);
                     PlanarListFn lf = planar_list_h(hc, vc);              // tiles with transparency (none for photos / video)
@@ -1556,9 +1251,9 @@ int launch_scale(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int fmt
                 return B200TIMG_OK;
             }
         }
-        if (pl->h.widest <= 8 && pl->v.widest <= 8 && !getenv("B200TIMG_NO_FIXED")) {
+        if (pl->h.widest <= 8 && pl->v.widest <= 8) {
             const int hc = fixed_class(pl->h.widest), vc = fixed_class(pl->v.widest);
-            const FixedVariant fv = pl->vertical_first ? fixed_h<true>(hc, vc, 'A') : fixed_h<false>(hc, vc, 'A');
+            const FixedVariant fv = pl->vertical_first ? fixed_h<true>(hc, vc) : fixed_h<false>(hc, vc);
             const int FTHv = fv.th;
             const int ntx = (ow + FTW - 1) / FTW, nty = (oh + FTHv - 1) / FTHv;
             std::vector<int32_t> tix(ntx), tiy(nty);
@@ -1590,105 +1285,66 @@ int launch_scale(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int fmt
                 return B200TIMG_OK;
             }
         }
-        if (!getenv("B200TIMG_NO_TWOPASS")) {
-            // long filters: two 1-D passes over a float4 intermediate in global memory
-            const size_t t_elems = pl->vertical_first ? (size_t)oh * iw : (size_t)ih * ow;
-            const size_t o_tmp = 0, o_flag = (sizeof(float4) * t_elems * n_frames + 255) / 256 * 256;
-            const size_t o_mask = o_flag + (sizeof(int) * (size_t)n_frames + 255) / 256 * 256;
-            B2_CUDA(ctx, ctx->scale_tmp.reserve(o_mask + (size_t)ow * oh * n_frames));
-            char *tb = ctx->scale_tmp.as<char>();
-            TwoPassParams T;
-            T.P = P; T.tmp = reinterpret_cast<float4 *>(tb + o_tmp); T.need_plain = reinterpret_cast<int *>(tb + o_flag);
-            T.mask = reinterpret_cast<unsigned char *>(tb + o_mask);
-            B2_CUDA(ctx, cudaMemsetAsync(T.need_plain, 0, sizeof(int) * (size_t)n_frames, ctx->stream));
-            const dim3 g2((ow + 31) / 32, (oh + 7) / 8, n_frames);
-            for (int plain = 0; plain < 2; ++plain) {
-                if (pl->vertical_first) {
-                    const dim3 g1((iw + 255) / 256, oh, n_frames);
-                    B2_KERNEL(ctx, plain ? "twopass_plain_kernels" : "twopass_v1_kernel");
-                    if (plain) twopass_v1_kernel<true><<<g1, 256, 0, ctx->stream>>>(in, T); else twopass_v1_kernel<false><<<g1, 256, 0, ctx->stream>>>(in, T);
-                    B2_LAUNCH_CHECK(ctx);
-                    B2_KERNEL(ctx, plain ? "twopass_plain_kernels" : "twopass_2_kernel");
-                    if (plain) twopass_2_kernel<true, true><<<g2, 256, 0, ctx->stream>>>(out, T); else twopass_2_kernel<true, false><<<g2, 256, 0, ctx->stream>>>(out, T);
-                    B2_LAUNCH_CHECK(ctx);
-                } else {
-                    const dim3 g1((ow + 31) / 32, (ih + 7) / 8, n_frames);
-                    // staged variant: window of a 32-column tile = first[tile start] .. max(first + count) over the tile
-                    H1sGeom HG{1, pl->h.widest | 1};
-                    for (int x0 = 0; x0 < ow; x0 += 32) {
-                        int hi = 0;
-                        for (int x = x0; x < std::min(ow, x0 + 32); ++x) hi = std::max(hi, pl->h.first[x] + pl->h.count[x]);
-                        HG.nwin = std::max(HG.nwin, hi - pl->h.first[x0]);
-                    }
-                    const size_t h1smem = sizeof(float4) * 8 * (size_t)HG.nwin + sizeof(float) * 32 * (size_t)HG.cpitch;
-                    B2_KERNEL(ctx, plain ? "twopass_plain_kernels" : "twopass_h1_kernel");
-                    // staging pays when the 32-column tiles are mostly full (4K -> 337 columns); with 67 columns the third
-                    // tile stages a whole window for 3 outputs: plain kernel
-                    const bool tiles_full = (long long)((ow + 31) / 32) * 32 * 100 <= (long long)ow * 115;
-                    if (h1smem <= 72 * 1024 && tiles_full && !getenv("B200TIMG_NO_H1S")) {
-                        if (plain) {
-                            B2_CUDA(ctx, cudaFuncSetAttribute(twopass_h1s_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 72 * 1024));
-                            twopass_h1s_kernel<true><<<g1, 256, h1smem, ctx->stream>>>(in, T, HG);
-                        } else {
-                            B2_CUDA(ctx, cudaFuncSetAttribute(twopass_h1s_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 72 * 1024));
-                            twopass_h1s_kernel<false><<<g1, 256, h1smem, ctx->stream>>>(in, T, HG);
-                        }
-                    } else if (!tiles_full && ow <= 4096 && n_frames <= 65535 && !getenv("B200TIMG_NO_H1F")) {
-                        // few output columns: flat (row, column) mapping; rows per CTA chosen so that rows x ow fills whole 256-thread rounds
-                        int rows = 8; double best = 0.0;
-                        for (int r = 4; r <= 64; ++r) {
-                            const long long items = (long long)r * ow, slots = (items + 255) / 256 * 256;
-                            const double fill = (double)items / (double)slots;
-                            if (fill > best + 1e-9) { best = fill; rows = r; }
-                        }
-                        const dim3 gf((ih + rows - 1) / rows, n_frames);
-                        if (plain) twopass_h1f_kernel<true><<<gf, 256, 0, ctx->stream>>>(in, T, rows); else twopass_h1f_kernel<false><<<gf, 256, 0, ctx->stream>>>(in, T, rows);
-                    } else if (plain) twopass_h1_kernel<true><<<g1, 256, 0, ctx->stream>>>(in, T); else twopass_h1_kernel<false><<<g1, 256, 0, ctx->stream>>>(in, T);
-                    B2_LAUNCH_CHECK(ctx);
-                    B2_KERNEL(ctx, plain ? "twopass_plain_kernels" : "twopass_2_kernel");
-                    if (plain) twopass_2_kernel<false, true><<<g2, 256, 0, ctx->stream>>>(out, T); else twopass_2_kernel<false, false><<<g2, 256, 0, ctx->stream>>>(out, T);
-                    B2_LAUNCH_CHECK(ctx);
+        // long filters: two 1-D passes over a float4 intermediate in global memory
+        const size_t t_elems = pl->vertical_first ? (size_t)oh * iw : (size_t)ih * ow;
+        const size_t o_tmp = 0, o_flag = (sizeof(float4) * t_elems * n_frames + 255) / 256 * 256;
+        const size_t o_mask = o_flag + (sizeof(int) * (size_t)n_frames + 255) / 256 * 256;
+        B2_CUDA(ctx, ctx->scale_tmp.reserve(o_mask + (size_t)ow * oh * n_frames));
+        char *tb = ctx->scale_tmp.as<char>();
+        TwoPassParams T;
+        T.P = P; T.tmp = reinterpret_cast<float4 *>(tb + o_tmp); T.need_plain = reinterpret_cast<int *>(tb + o_flag);
+        T.mask = reinterpret_cast<unsigned char *>(tb + o_mask);
+        B2_CUDA(ctx, cudaMemsetAsync(T.need_plain, 0, sizeof(int) * (size_t)n_frames, ctx->stream));
+        const dim3 g2((ow + 31) / 32, (oh + 7) / 8, n_frames);
+        for (int plain = 0; plain < 2; ++plain) {
+            if (pl->vertical_first) {
+                const dim3 g1((iw + 255) / 256, oh, n_frames);
+                B2_KERNEL(ctx, plain ? "twopass_plain_kernels" : "twopass_v1_kernel");
+                if (plain) twopass_v1_kernel<true><<<g1, 256, 0, ctx->stream>>>(in, T); else twopass_v1_kernel<false><<<g1, 256, 0, ctx->stream>>>(in, T);
+                B2_LAUNCH_CHECK(ctx);
+                B2_KERNEL(ctx, plain ? "twopass_plain_kernels" : "twopass_2_kernel");
+                if (plain) twopass_2_kernel<true, true><<<g2, 256, 0, ctx->stream>>>(out, T); else twopass_2_kernel<true, false><<<g2, 256, 0, ctx->stream>>>(out, T);
+                B2_LAUNCH_CHECK(ctx);
+            } else {
+                const dim3 g1((ow + 31) / 32, (ih + 7) / 8, n_frames);
+                // staged variant: window of a 32-column tile = first[tile start] .. max(first + count) over the tile
+                H1sGeom HG{1, pl->h.widest | 1};
+                for (int x0 = 0; x0 < ow; x0 += 32) {
+                    int hi = 0;
+                    for (int x = x0; x < std::min(ow, x0 + 32); ++x) hi = std::max(hi, pl->h.first[x] + pl->h.count[x]);
+                    HG.nwin = std::max(HG.nwin, hi - pl->h.first[x0]);
                 }
+                const size_t h1smem = sizeof(float4) * 8 * (size_t)HG.nwin + sizeof(float) * 32 * (size_t)HG.cpitch;
+                B2_KERNEL(ctx, plain ? "twopass_plain_kernels" : "twopass_h1_kernel");
+                // staging pays when the 32-column tiles are mostly full (4K -> 337 columns); with 67 columns the third
+                // tile stages a whole window for 3 outputs: plain kernel
+                const bool tiles_full = (long long)((ow + 31) / 32) * 32 * 100 <= (long long)ow * 115;
+                if (h1smem <= 72 * 1024 && tiles_full && !getenv("B200TIMG_NO_H1S")) {
+                    if (plain) {
+                        B2_CUDA(ctx, cudaFuncSetAttribute(twopass_h1s_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 72 * 1024));
+                        twopass_h1s_kernel<true><<<g1, 256, h1smem, ctx->stream>>>(in, T, HG);
+                    } else {
+                        B2_CUDA(ctx, cudaFuncSetAttribute(twopass_h1s_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 72 * 1024));
+                        twopass_h1s_kernel<false><<<g1, 256, h1smem, ctx->stream>>>(in, T, HG);
+                    }
+                } else if (!tiles_full && ow <= 4096 && n_frames <= 65535 && !getenv("B200TIMG_NO_H1F")) {
+                    // few output columns: flat (row, column) mapping; rows per CTA chosen so that rows x ow fills whole 256-thread rounds
+                    int rows = 8; double best = 0.0;
+                    for (int r = 4; r <= 64; ++r) {
+                        const long long items = (long long)r * ow, slots = (items + 255) / 256 * 256;
+                        const double fill = (double)items / (double)slots;
+                        if (fill > best + 1e-9) { best = fill; rows = r; }
+                    }
+                    const dim3 gf((ih + rows - 1) / rows, n_frames);
+                    if (plain) twopass_h1f_kernel<true><<<gf, 256, 0, ctx->stream>>>(in, T, rows); else twopass_h1f_kernel<false><<<gf, 256, 0, ctx->stream>>>(in, T, rows);
+                } else if (plain) twopass_h1_kernel<true><<<g1, 256, 0, ctx->stream>>>(in, T); else twopass_h1_kernel<false><<<g1, 256, 0, ctx->stream>>>(in, T);
+                B2_LAUNCH_CHECK(ctx);
+                B2_KERNEL(ctx, plain ? "twopass_plain_kernels" : "twopass_2_kernel");
+                if (plain) twopass_2_kernel<false, true><<<g2, 256, 0, ctx->stream>>>(out, T); else twopass_2_kernel<false, false><<<g2, 256, 0, ctx->stream>>>(out, T);
+                B2_LAUNCH_CHECK(ctx);
             }
-            return B200TIMG_OK;
         }
-        // tile shape: largest of a few candidates whose decoded window + intermediate fit in shared memory
-        static const int cand[][2] = {{64, 16}, {32, 16}, {32, 8}, {16, 8}, {8, 4}};
-        TileGeom G{0, 0, 0, 0};
-        size_t smem = 0;
-        size_t smem_budget = 74 * 1024;      // 3 CTAs/SM
-        if (const char *e = getenv("B200TIMG_TILE_SMEM_KB")) smem_budget = (size_t)atoi(e) * 1024;   // tuning knob
-        for (const auto &c : cand) {
-            int nix = 1, niy = 1;
-            for (int x0 = 0; x0 < ow; x0 += c[0]) {
-                int lo = 0x7fffffff, hi = -1;
-                for (int x = x0; x < std::min(ow, x0 + c[0]); ++x) { lo = std::min(lo, pl->h.first[x]); hi = std::max(hi, pl->h.first[x] + pl->h.count[x] - 1); }
-                nix = std::max(nix, hi - lo + 1);
-            }
-            for (int y0 = 0; y0 < oh; y0 += c[1]) {
-                int lo = 0x7fffffff, hi = -1;
-                for (int y = y0; y < std::min(oh, y0 + c[1]); ++y) { lo = std::min(lo, pl->v.first[y]); hi = std::max(hi, pl->v.first[y] + pl->v.count[y] - 1); }
-                niy = std::max(niy, hi - lo + 1);
-            }
-            const size_t need = sizeof(float4) * ((size_t)nix * niy + (pl->vertical_first ? (size_t)c[1] * nix : (size_t)niy * c[0]))
-                              + sizeof(int) * (2 * (size_t)c[0] + 2 * (size_t)c[1])
-                              + sizeof(float) * ((size_t)c[0] * (pl->h.widest | 1) + (size_t)c[1] * (pl->v.widest | 1));
-            if (need <= smem_budget || (&c == &cand[4] && need <= 200 * 1024)) { G = TileGeom{c[0], c[1], nix, niy}; smem = need; break; }
-        }
-        if (G.tw) {
-            TiledFn fn = pl->vertical_first ? pick_h<true>(tap_class(pl->h.widest), tap_class(pl->v.widest))
-                                            : pick_h<false>(tap_class(pl->h.widest), tap_class(pl->v.widest));
-            B2_CUDA(ctx, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-            const dim3 grid((ow + G.tw - 1) / G.tw, (oh + G.th - 1) / G.th, n_frames);
-            B2_KERNEL(ctx, "resample_tiled_kernel");
-            fn<<<grid, RT, smem, ctx->stream>>>(in, out, P, G);
-        } else {
-            // extreme ratios whose window does not fit in shared memory: per-pixel kernel
-            const dim3 grid((ow + 31) / 32, (oh + 7) / 8, n_frames);
-            B2_KERNEL(ctx, "resample_direct_kernel");
-            if (pl->vertical_first) resample_direct_kernel<true><<<grid, 256, 0, ctx->stream>>>(in, out, P);
-            else resample_direct_kernel<false><<<grid, 256, 0, ctx->stream>>>(in, out, P);
-        }
+        return B200TIMG_OK;
     }
     B2_LAUNCH_CHECK(ctx);
     return B200TIMG_OK;

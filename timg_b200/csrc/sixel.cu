@@ -20,10 +20,11 @@
 //   sixel_palette_kernel   1 CTA : sampled histogram (packed u16 smem atomics) -> compaction ->
 //                                  median cut (stable counting sort by 5-bit key, block scans)
 //   sixel_lut_kernel       32 CTAs: 32768-entry nearest-colour table
-//   sixel_dither_kernel    1 CTA : FS wavefront; a warp owns a band of 32 rows with a 2-column
-//                                  skew between lanes (errors handed down by shuffle), bands are
-//                                  pipelined warp to warp through a boundary row + progress flag
-//   sixel_emit_kernel<0/1> 1 CTA per 6-row band: sizes, then bytes (per-colour RLE rows)
+//   sixel_map_kernel       frames without diffusion: table lookup per pixel
+//   sixel_dither2_kernel   (sixel_dither.cu) FS wavefront for frames with diffusion
+//   sixel_emit5_kernel     1 CTA per 6-row band: sort, then bytes (per-colour RLE rows) into a scratch slot; frames wider
+//                          than 4095 px take the single-pass sixel_emit2_kernel (sixel_emit.cu) instead
+//   sixel_layout_kernel, sixel_sizes_to_offsets_kernel, sixel_compact_kernel: band offsets, frame offsets, final bytes
 // Algorithmic bytes per frame: 4*W*H read + encoded bytes written; index plane (1 B/px), boundary
 // rows, LUT and tables are intermediates.
 #include <cstdlib>
@@ -454,191 +455,9 @@ sixel_map_kernel(const uint32_t *__restrict__ fb, long long npix, SixelWork W, t
         W.index[g.idx0() + i] = lut[hash15(fb[g.px0() + i])];
 }
 
-// ---- Floyd-Steinberg wavefront --------------------------------------------------------------
-constexpr uint32_t EZ = 256u | (256u << 9) | (256u << 18);     // packed zero error (each channel biased by 256)
-__device__ __forceinline__ int fs_tap(int v, int e, int k) {      // error_diffuse(): c = v + e*k/16, clamp
-    const int t = e * k;
-    const int q = (t + ((t >> 31) & 15)) >> 4;                  // C division truncates toward zero
-    return min(255, max(0, v + q));
-}
-// One pixel's quantisation error, unpacked: e[c] in [-255,255] and bias[c] = (e<0 ? 15 : 0), so that
-// error_diffuse()'s  e*k/16 (C truncation)  is  (e*k + bias) >> 4  -- one IMAD and one shift per tap.
-struct FsErr {
-    int e[3], b[3];
-    __device__ __forceinline__ void zero() { e[0] = e[1] = e[2] = 0; b[0] = b[1] = b[2] = 0; }
-    __device__ __forceinline__ void set(int r, int g, int bl) {
-        e[0] = r; e[1] = g; e[2] = bl;
-        b[0] = (r >> 31) & 15; b[1] = (g >> 31) & 15; b[2] = (bl >> 31) & 15;
-    }
-    __device__ __forceinline__ void unpack(uint32_t p) { set((int)(p & 511) - 256, (int)((p >> 9) & 511) - 256, (int)((p >> 18) & 511) - 256); }
-    __device__ __forceinline__ uint32_t pack() const { return (uint32_t)(e[0] + 256) | ((uint32_t)(e[1] + 256) << 9) | ((uint32_t)(e[2] + 256) << 18); }
-};
-__device__ __forceinline__ int fs_add(int v, const FsErr &er, int c, int k) {
-    return min(255, max(0, v + ((er.e[c] * k + er.b[c]) >> 4)));
-}
-constexpr int DW_MAX = 24;     // warps per frame CTA (upper bound; the launch picks how many)
-constexpr int DCH = 16;        // columns per staged chunk
-constexpr int DIN_STRIDE = DCH + 1;              // u32 words per staged row (odd: lanes hit distinct banks)
-constexpr int DOUT_STRIDE = 20;                  // bytes per staged output row (5 words: conflict-free)
-constexpr int DWARP_SMEM = 2 * 32 * DIN_STRIDE * 4 + 32 * DOUT_STRIDE;   // per warp
-
-// A warp owns a band of 32 rows; lane l runs row band*32+l two columns behind lane l-1, so the three
-// errors it needs from the row above arrive by one shuffle per step.  Pixels are staged through
-// shared memory in chunks of DCH steps, pre-skewed (row r of the tile starts at column base-2r) and
-// loaded/stored by half-warps so global traffic is 64-byte segments instead of 32 scattered lines.
-// Consecutive bands are pipelined through a boundary row of packed errors in global memory (L2)
-// plus a per-band progress counter in shared memory.
-__global__ void __launch_bounds__(DW_MAX * 32)
-sixel_dither_kernel(const uint32_t *__restrict__ fb, int w, int h, int nwarps, SixelWork W) {
-    extern __shared__ __align__(16) uint8_t s_dyn[];              // lut[32768] | per-warp tiles
-    __shared__ uint32_t s_pal[256];
-    __shared__ volatile int s_progress[2048];                     // columns completed by each band's last row
-    const int f = blockIdx.x;
-    const SixelFrameHdr *hdr = W.hdr + f;
-    if (!hdr->diffuse) return;
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    const int nthreads = nwarps * 32;
-    uint8_t *s_lut = s_dyn;
-    for (int i = tid; i < 32768 / 4; i += nthreads)
-        reinterpret_cast<uint32_t *>(s_lut)[i] = reinterpret_cast<const uint32_t *>(W.lut + (long long)f * 32768)[i];
-    for (int i = tid; i < 256; i += nthreads) s_pal[i] = hdr->palette[i];     // nthreads may be < 256
-    for (int i = tid; i < W.nb32; i += nthreads) s_progress[i] = 0;
-    __syncthreads();
-    uint32_t *s_in = reinterpret_cast<uint32_t *>(s_dyn + 32768 + (size_t)wid * DWARP_SMEM);   // [2][32][DIN_STRIDE]
-    uint8_t *s_out = reinterpret_cast<uint8_t *>(s_in + 2 * 32 * DIN_STRIDE);                    // [32][DOUT_STRIDE]
-    const uint32_t *frame = fb + (long long)f * w * h;
-    uint8_t *index = W.index + (long long)f * w * h;
-    uint32_t *bnd = W.boundary + (long long)f * W.nb32 * w;
-    const int hrow = lane >> 4, hcol = lane & 15;                 // half-warp staging coordinates
-
-    for (int band = wid; band < W.nb32; band += nwarps) {
-        const int y = band * 32 + lane;
-        const bool row_ok = y < h;
-        const bool last_row = (y == h - 1);
-        const uint32_t *bin = band > 0 ? bnd + (long long)(band - 1) * w : nullptr;
-        uint32_t *bout = bnd + (long long)band * w;
-        uint32_t last_e = EZ;
-        FsErr up_m1, up_0, up_p1, own, e_first;
-        up_m1.zero(); up_0.zero(); up_p1.zero(); own.zero(); e_first.zero();
-        const int steps = w + 62, nchunks = (steps + DCH - 1) / DCH;
-        // pre-skewed load of chunk c into registers: element i covers tile row 2i+hrow, column hcol
-        uint32_t pre[16];
-        auto load_chunk = [&](int c) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-                const int r = 2 * i + hrow, yy = band * 32 + r, x = c * DCH - 2 * r + hcol;
-                pre[i] = (yy < h && x >= 0 && x < w) ? frame[(long long)yy * w + x] : 0u;
-            }
-        };
-        auto store_chunk = [&](int c) {
-            uint32_t *t = s_in + (c & 1) * 32 * DIN_STRIDE;
-#pragma unroll
-            for (int i = 0; i < 16; ++i) t[(2 * i + hrow) * DIN_STRIDE + hcol] = pre[i];
-        };
-        load_chunk(0); store_chunk(0);
-        __syncwarp();
-        for (int c = 0; c < nchunks; ++c) {
-            const int t0 = c * DCH;
-            if (c + 1 < nchunks) load_chunk(c + 1);                // in flight while this chunk computes
-            uint32_t binreg = EZ;
-            if (band > 0) {                                       // stay behind the previous band's last row
-                const int need = min(w, t0 + DCH + 1);
-                if (lane == 0) { while (s_progress[band - 1] < need) __nanosleep(32); __threadfence_block(); }
-                __syncwarp();
-                const int bx = t0 + 1 + lane;                     // lane 0 consumes bin[t+1] at step t
-                if (lane < DCH && bx < w) binreg = __ldcg(bin + bx);
-                if (c == 0 && lane == 0) up_p1.unpack(__ldcg(bin));   // e(0, y-1): lane 0 has no warm-up step
-            }
-            const uint32_t *tin = s_in + (c & 1) * 32 * DIN_STRIDE + lane * DIN_STRIDE;
-            uint32_t bkeep = EZ;
-            // interior chunk: every lane is strictly inside its row for all DCH steps and no lane runs the
-            // frame's last row -> the step needs no range checks and always diffuses
-            const bool interior = (t0 - 62 >= 1) && (t0 + DCH - 1 <= w - 2) && (band * 32 + 31 < h - 1);
-            if (interior) {
-#pragma unroll 4
-                for (int j = 0; j < DCH; ++j) {
-                    uint32_t recv = __shfl_up_sync(0xffffffffu, last_e, 1);
-                    const uint32_t b0 = __shfl_sync(0xffffffffu, binreg, j);
-                    if (lane == 0) recv = b0;
-                    up_m1 = up_0; up_0 = up_p1; up_p1.unpack(recv);
-                    const uint32_t px = tin[j];
-                    int v[3] = {(int)(px & 0xff), (int)((px >> 8) & 0xff), (int)((px >> 16) & 0xff)};
-#pragma unroll
-                    for (int ch = 0; ch < 3; ++ch) {
-                        v[ch] = fs_add(v[ch], up_m1, ch, 1);
-                        v[ch] = fs_add(v[ch], up_0, ch, 5);
-                        v[ch] = fs_add(v[ch], up_p1, ch, 3);
-                        v[ch] = fs_add(v[ch], own, ch, 7);
-                    }
-                    const uint32_t cell = ((uint32_t)(v[0] >> 3) << 10) | ((uint32_t)(v[1] >> 3) << 5) | (uint32_t)(v[2] >> 3);
-                    const uint32_t ci = s_lut[cell];
-                    const uint32_t pal = s_pal[ci];
-                    own.set(v[0] - (int)(pal & 0xff), v[1] - (int)((pal >> 8) & 0xff), v[2] - (int)((pal >> 16) & 0xff));
-                    last_e = own.pack();
-                    s_out[lane * DOUT_STRIDE + j] = (uint8_t)ci;
-                    const uint32_t e31 = __shfl_sync(0xffffffffu, last_e, 31);
-                    if (lane == j) bkeep = e31;
-                }
-            } else {
-#pragma unroll 2
-                for (int j = 0; j < DCH; ++j) {
-                    const int t = t0 + j, x = t - 2 * lane;
-                    uint32_t recv = __shfl_up_sync(0xffffffffu, last_e, 1);
-                    const uint32_t b0 = __shfl_sync(0xffffffffu, binreg, j);
-                    if (lane == 0) recv = b0;
-                    up_m1 = up_0; up_0 = up_p1; up_p1.unpack(recv);
-                    uint32_t ci = 0;
-                    if (x >= 0 && x < w && row_ok) {
-                        const uint32_t px = tin[j];
-                        int v[3] = {(int)(px & 0xff), (int)((px >> 8) & 0xff), (int)((px >> 16) & 0xff)};
-#pragma unroll
-                        for (int ch = 0; ch < 3; ++ch) {
-                            v[ch] = fs_add(v[ch], up_m1, ch, 1);                       // from (x-1, y-1)
-                            v[ch] = fs_add(v[ch], up_0, ch, 5);                        // from (x,   y-1)
-                            v[ch] = fs_add(v[ch], up_p1, ch, 3);                       // from (x+1, y-1)
-                            if (x == w - 1) v[ch] = fs_add(v[ch], e_first, ch, 3);     // libsixel: (0,y)'s below-left tap
-                            v[ch] = fs_add(v[ch], own, ch, 7);                         // from (x-1, y)
-                        }
-                        const uint32_t cell = ((uint32_t)(v[0] >> 3) << 10) | ((uint32_t)(v[1] >> 3) << 5) | (uint32_t)(v[2] >> 3);
-                        ci = s_lut[cell];
-                        const uint32_t pal = s_pal[ci];
-                        if (x < w - 1 && !last_row) own.set(v[0] - (int)(pal & 0xff), v[1] - (int)((pal >> 8) & 0xff), v[2] - (int)((pal >> 16) & 0xff));
-                        else own.zero();
-                        if (x == 0) e_first = own;
-                        last_e = own.pack();
-                    } else if (x >= w) {
-                        last_e = EZ;
-                    }
-                    s_out[lane * DOUT_STRIDE + j] = (uint8_t)ci;
-                    const uint32_t e31 = __shfl_sync(0xffffffffu, last_e, 31);      // the band's last row, column t-62
-                    if (lane == j) bkeep = e31;
-                }
-            }
-            __syncwarp();
-            // write this chunk's indices: half-warp per row, 16 contiguous bytes
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-                const int r = 2 * i + hrow, yy = band * 32 + r, x = t0 - 2 * r + hcol;
-                if (yy < h && x >= 0 && x < w) index[(long long)yy * w + x] = s_out[r * DOUT_STRIDE + hcol];
-            }
-            {   // boundary row for the next band, then publish progress
-                const int x = t0 + lane - 62;
-                if (lane < DCH && x >= 0 && x < w) __stcg(bout + x, bkeep);
-                __threadfence_block();                            // every storing lane orders its own store ...
-                __syncwarp();                                     // ... before lane 0 raises the flag
-                const int done = min(w, t0 + DCH - 62);
-                if (lane == 0 && done > 0) s_progress[band] = done;
-            }
-            if (c + 1 < nchunks) store_chunk(c + 1);
-            __syncwarp();
-        }
-    }
-}
-
 // ---- emit ------------------------------------------------------------------------------------
 // Branch-light formatting for values < 10000 (run lengths, gaps and colour numbers are bounded by
 // the frame width <= 4095 and 255): no loops, so lanes of a warp do not serialise on digit counts.
-__device__ __forceinline__ uint32_t ndig4(uint32_t v) { return 1u + (v >= 10u) + (v >= 100u) + (v >= 1000u); }
 __device__ __forceinline__ char *put_num4(char *o, uint32_t v) {
     const uint32_t d3 = v / 1000u, r3 = v - d3 * 1000u, d2 = r3 / 100u, r2 = r3 - d2 * 100u, d1 = r2 / 10u, d0 = r2 - d1 * 10u;
     if (v >= 1000u) *o++ = (char)('0' + d3);
@@ -647,8 +466,7 @@ __device__ __forceinline__ char *put_num4(char *o, uint32_t v) {
     *o++ = (char)('0' + d0);
     return o;
 }
-__device__ __forceinline__ uint32_t rle_len(uint32_t n) { return n > 3u ? 2u + ndig4(n) : n; }   // tosixel.c sixel_put_flash
-__device__ __forceinline__ char *put_rle(char *o, uint32_t n, char ch) {
+__device__ __forceinline__ char *put_rle(char *o, uint32_t n, char ch) {     // tosixel.c sixel_put_flash
     if (n > 3u) { *o++ = '!'; o = put_num4(o, n); *o++ = ch; }
     else { if (n > 0u) *o++ = ch; if (n > 1u) *o++ = ch; if (n > 2u) *o++ = ch; }
     return o;
@@ -682,96 +500,15 @@ __device__ __forceinline__ void walk_runs(const uint32_t *sorted, int lo, int hi
     }
 }
 
-// One CTA per 6-row band.  (1) per-warp counting sort of the band's (colour, x, bits) entries by
-// colour -- warps own contiguous column ranges, so warp-major order is x order and the sort is
-// stable; (2) every run head sizes its "gap + run" bytes, block scan -> offsets; (3) WRITE: bytes.
-__global__ void __launch_bounds__(ET)
-sixel_emit_kernel(EmitGeom G, SixelWork W) {
-    extern __shared__ uint32_t s_sorted[];                   // [6*w]
-    __shared__ uint32_t s_cnt[EW][256];
-    __shared__ uint32_t s_mask[EW * 256];
-    __shared__ uint32_t s_w[ET / 32];
-    const int band = blockIdx.x, f = blockIdx.y, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    const int w = G.w;
-    const SixelFrameHdr *hdr = W.hdr + f;
-    const uint8_t *idx = W.index + ((long long)f * G.h + (long long)band * 6) * w;
-
-    for (int i = tid; i < EW * 256; i += ET) { (&s_cnt[0][0])[i] = 0; s_mask[i] = 0; }
-    __syncthreads();
-
-    // (1a) count entries per (warp, colour): shared-memory atomics, a few per column
-    const int x_lo = wid * G.cols_per_warp, x_hi = min(w, x_lo + G.cols_per_warp);
-    uint32_t *cnt = s_cnt[wid];
-    for (int x = x_lo + lane; x < x_hi; x += 32) {
-        uint32_t col[6], bits[6];
-        const uint32_t valid = column_entries(idx, w, x, col, bits);
-#pragma unroll
-        for (int s = 0; s < 6; ++s) if (valid & (1u << s)) atomicAdd(&cnt[col[s]], 1u);
-    }
-    __syncthreads();
-    // per-colour totals -> colour bases -> per (warp, colour) start offsets (in place)
-    uint32_t tot_c = 0;
-    if (tid < 256) for (int k = 0; k < EW; ++k) tot_c += s_cnt[k][tid];
-    uint32_t n_ent; const uint32_t cb = block_excl_scan<ET>(tid < 256 ? tot_c : 0, s_w, n_ent);
-    if (tid < 256) {
-        uint32_t run = cb;
-        for (int k = 0; k < EW; ++k) { const uint32_t v = s_cnt[k][tid]; s_cnt[k][tid] = run; run += v; }
-    }
-    __syncthreads();
-    // (1b) scatter.  Ranks must follow x: per 32-column step the lanes holding each colour are
-    // collected in a per-warp mask table (one atomicOr per entry); an entry's rank is the number of
-    // lower lanes in its colour's mask, and the lowest lane advances the (warp, colour) cursor.
-    uint32_t *M = s_mask + wid * 256;
-    const uint32_t lt = (1u << lane) - 1;
-    for (int x0 = x_lo; x0 < x_hi; x0 += 32) {
-        const int x = x0 + lane;
-        uint32_t col[6], bits[6];
-        const uint32_t valid = x < x_hi ? column_entries(idx, w, x, col, bits) : 0u;
-#pragma unroll
-        for (int s = 0; s < 6; ++s) if (valid & (1u << s)) atomicOr(&M[col[s]], 1u << lane);
-        __syncwarp();
-        uint32_t mk[6];
-#pragma unroll
-        for (int s = 0; s < 6; ++s)
-            if (valid & (1u << s)) {
-                mk[s] = M[col[s]];
-                s_sorted[cnt[col[s]] + __popc(mk[s] & lt)] = ent_pack(col[s], (uint32_t)x, bits[s]);
-            }
-        __syncwarp();
-#pragma unroll
-        for (int s = 0; s < 6; ++s)
-            if ((valid & (1u << s)) && (mk[s] & lt) == 0) { cnt[col[s]] += (uint32_t)__popc(mk[s]); M[col[s]] = 0; }
-        __syncwarp();
-    }
-    __syncthreads();
-    // (2) sizes
-    const int n = (int)n_ent;
-    const uint32_t minc = s_sorted[0] >> 18;
-    const int per = (n + ET - 1) / ET, lo = min(n, tid * per), hi = min(n, lo + per);
-    uint32_t local = 0;
-    walk_runs(s_sorted, lo, hi, n, [&](uint32_t c, uint32_t, uint32_t gap, uint32_t len, bool first) {
-        local += rle_len(gap) + rle_len(len) + (first ? 1u + ndig4(c) + (c != minc ? 1u : 0u) : 0u);
-    });
-    uint32_t band_total; uint32_t at = block_excl_scan<ET>(local, s_w, band_total);
-    if (tid == 0) W.band_bytes[(long long)f * W.nbands + band] = band_total;
-    // (3) bytes, into this band's scratch slot (compacted into the final stream later)
-    char *o = W.scratch + ((size_t)f * W.nbands + band) * W.band_cap + at;
-    walk_runs(s_sorted, lo, hi, n, [&](uint32_t c, uint32_t bits, uint32_t gap, uint32_t len, bool first) {
-        if (first) { if (c != minc) *o++ = '$'; *o++ = '#'; o = put_num4(o, c); }
-        o = put_rle(o, gap, '?');
-        o = put_rle(o, len, (char)('?' + bits));
-    });
-}
-
-// ---- emit v1b: one walk instead of two -------------------------------------------------------------------------------
-// Per-line instruction counts show v1 spending a large share of its instructions in the sizes walk and in the byte-wise,
-// heavily divergent formatting of the write walk (every lane of a warp sits in another branch of put_rle / put_num4 and
-// stores single bytes to global memory).  v1b walks the sorted entries ONCE: every run head builds its <= 3 pieces
-// (colour introducer, gap, run) as 64-bit values with branch-light arithmetic and appends them to a thread-private slot
-// in shared memory (word-interleaved over the threads, so the stores are conflict-free; the <= 3 words a piece touches
-// are all stored, no branches); the slot's fill IS the thread's size, and after the block scan the slot is copied out with
-// aligned 4-byte stores.  The slots take over the sort's count/mask tables.  A thread whose bytes do not fit its slot
-// (noise frames) falls back to v1's write walk for its own range.
+// ---- emit5: one CTA per 6-row band -----------------------------------------------------------------------------------
+// (1) a per-warp counting sort of the band's (colour, x, bits) entries by colour: warps own contiguous column ranges, so
+// warp-major order is x order and the sort is stable.  (2) ONE walk over the sorted entries: every run head builds its
+// <= 3 pieces (colour introducer, gap, run) as 64-bit values with branch-light arithmetic and appends them to a
+// thread-private slot in shared memory (word-interleaved over the threads, so the stores are conflict-free; the <= 3 words
+// a piece touches are all stored, no branches); the slot's fill IS the thread's size.  (3) after the block scan the slots
+// are copied out.  The slots take over the sort's count/mask tables.  A thread whose bytes do not fit its slot (noise
+// frames) writes its own range byte by byte with put_rle / put_num4 instead.  The walk replaced a sizes walk plus a
+// byte-wise write walk, which per-line instruction counts showed spending most of the instructions of an earlier emitter.
 constexpr int SLOT_WORDS = 22;                   // words of a slot
 constexpr int STASH_STEPS = 6;                   // 32-column steps of a warp whose column entries stay in registers (w <= 3072)
 constexpr uint32_t SLOT_MAX = 4 * (SLOT_WORDS - 3);   // an append may START at byte <= SLOT_MAX (it touches <= 3 words)
@@ -819,31 +556,31 @@ __device__ __forceinline__ void slot_append(uint32_t *slot, uint32_t &pos, uint3
     pos = np;
 }
 
-// Phase clocks of the emit kernels (tools/bench_sixel_emit.py --clocks): built only with -DB200TIMG_EMIT_CLOCKS.  Thread 0
-// stamps clock64() after a CTA barrier at every phase boundary (the instrumented build adds barriers where a phase has
-// none) and adds the CTA's phase durations to g_emit_clocks[kernel][phase]; b200timg_emit_clocks() reads and clears them.
+// Phase clocks of emit5 (tools/bench_sixel_emit.py --clocks): built only with -DB200TIMG_EMIT_CLOCKS.  Thread 0 stamps
+// clock64() after a CTA barrier at every phase boundary (the instrumented build adds barriers where a phase has none) and
+// adds the CTA's phase durations to g_emit_clocks[phase]; b200timg_emit_clocks() reads and clears them.
 #ifdef B200TIMG_EMIT_CLOCKS
 constexpr int EMIT_CLK_PHASES = 8;
-__device__ unsigned long long g_emit_clocks[2][EMIT_CLK_PHASES];     // [0: emit1b, 1: emit5][phase], SM cycles summed over CTAs
+__device__ unsigned long long g_emit_clocks[EMIT_CLK_PHASES];        // SM cycles summed over CTAs
 #define EMIT_CLK_BEGIN long long clk_[EMIT_CLK_PHASES + 1]; int clk_n_ = 0; if (threadIdx.x == 0) clk_[clk_n_] = clock64(); ++clk_n_
 #define EMIT_CLK() do { __syncthreads(); if (threadIdx.x == 0) clk_[clk_n_] = clock64(); ++clk_n_; } while (0)
-#define EMIT_CLK_END(kern) do { if (threadIdx.x == 0) for (int k_ = 0; k_ + 1 < clk_n_; ++k_) \
-        atomicAdd(&g_emit_clocks[kern][k_], (unsigned long long)(clk_[k_ + 1] - clk_[k_])); } while (0)
+#define EMIT_CLK_END() do { if (threadIdx.x == 0) for (int k_ = 0; k_ + 1 < clk_n_; ++k_) \
+        atomicAdd(&g_emit_clocks[k_], (unsigned long long)(clk_[k_ + 1] - clk_[k_])); } while (0)
 #else
 #define EMIT_CLK_BEGIN do {} while (0)
 #define EMIT_CLK() do {} while (0)
-#define EMIT_CLK_END(kern) do {} while (0)
+#define EMIT_CLK_END() do {} while (0)
 #endif
 
-// emit5 (V5) is v1b with two changes, both chosen from v1b's phase clocks (DESIGN.md §5):
+// Two more choices of emit5, both taken from phase clocks (DESIGN.md §5):
 //   * the band's six index rows (one contiguous block of 6*w bytes) come in with coalesced word loads, all in flight at
 //     once and issued before the table zeroing, into the entry array (dead until the scatter); the count pass reads its
-//     columns from there.  v1b's count pass waited for one global round trip per 32-column step.  (w <= 3072 only: wider
-//     bands re-read their columns in the scatter pass, so they keep v1b's loads.)
+//     columns from there instead of waiting for one global round trip per 32-column step.  (w <= 3072 only: wider
+//     bands re-read their columns in the scatter pass.)
 //   * the copy-out: when no slot overflowed, every thread moves its slot's bytes to their place in one contiguous byte
 //     image of the band in shared memory (the entry array again), and the CTA writes that image to the 256-byte aligned
-//     scratch slot with 16-byte stores.  v1b's threads each stored their ~32 bytes as 4-byte words, a warp store touching
-//     32 sectors.
+//     scratch slot with 16-byte stores, instead of every thread storing its ~32 bytes as 4-byte words (a warp store
+//     touching 32 sectors).
 constexpr int ROW_WORDS = (6 * 32 * STASH_STEPS * EW + 3) / 4 / ET + 1;   // words of the staged rows per thread (+1: misalignment)
 
 // Band accessors (emit, compaction): the CTA's frame and 6-row band, where the band's index rows, size, offset and
@@ -882,9 +619,9 @@ struct BandMixed {                        // flat band blockIdx.x
     __device__ __forceinline__ size_t scr(const SixelWork &) const { return (size_t)D.scr + (size_t)band * D.band_cap; }
 };
 
-template <bool V5, class A>
+template <class A>
 __global__ void __launch_bounds__(ET, 2)
-sixel_emit1b_kernel(typename A::Params G, SixelWork W) {
+sixel_emit5_kernel(typename A::Params G, SixelWork W) {
     extern __shared__ uint32_t s_sorted[];                   // [6*w]
     __shared__ uint32_t s_tab[SLOT_WORDS * ET];              // sort: cnt[EW][256] | mask[EW][256]; afterwards: slots
     __shared__ uint32_t s_w[ET / 32];
@@ -895,7 +632,7 @@ sixel_emit1b_kernel(typename A::Params G, SixelWork W) {
     EMIT_CLK_BEGIN;
     const bool stash = a.cols_per_warp() <= 32 * STASH_STEPS;
     const uint8_t *cols = idx;                               // where the count pass reads the band's rows
-    if (V5 && stash) {
+    if (stash) {
         // aligned words covering [idx, idx + 6w).  The <= 3 bytes outside the band stay inside the index region: sixel_plan
         // starts it on a 256-byte boundary and pads its end to one (o_idx, align_up(npix * n_frames, 256)), so rounding
         // the first band's start down or the last band's end up to a word never leaves it.
@@ -913,9 +650,8 @@ sixel_emit1b_kernel(typename A::Params G, SixelWork W) {
         for (int i = tid; i < 2 * EW * 256; i += ET) s_tab[i] = 0;
     }
     __syncthreads();
-    if (!V5) EMIT_CLK();                                     // zero
-    // (1) the sort: as in v1, but the column entries (<= 6 distinct colours of a column with their row bits) are computed
-    // once: the count pass parks them in registers (3 words per 32-column step, steps unrolled) for the scatter pass
+    // (1) the sort.  The column entries (<= 6 distinct colours of a column with their row bits) are computed once: the
+    // count pass parks them in registers (3 words per 32-column step, steps unrolled) for the scatter pass
     const int x_lo = wid * a.cols_per_warp(), x_hi = min(w, x_lo + a.cols_per_warp());
     uint32_t *cnt = s_tab + wid * 256, *M = s_tab + EW * 256 + wid * 256;
     uint32_t k0[STASH_STEPS], k1[STASH_STEPS], k2[STASH_STEPS];     // colours 0-3 | colours 4-5, valid, bits 5 | bits 0-4
@@ -1023,8 +759,8 @@ sixel_emit1b_kernel(typename A::Params G, SixelWork W) {
     uint32_t band_total; const uint32_t at = block_excl_scan<ET>(local, s_w, band_total);
     if (tid == 0) W.band_bytes[a.slot(W)] = band_total;
     EMIT_CLK();                                              // scan
-    // (3) the slot's bytes to `at` of this band's 16-byte aligned scratch place (v1b), or of its image in shared memory
-    // (emit5): head bytes up to a word boundary, whole words realigned with a funnel shift, tail bytes
+    // (3) the slot's bytes to `at` of the band's image in shared memory, or of its 16-byte aligned scratch place: head
+    // bytes up to a word boundary, whole words realigned with a funnel shift, tail bytes
     char *const band_out = W.scratch + a.scr(W);
     char *o = band_out + at;
     auto slot_out = [&](char *d) {
@@ -1042,9 +778,9 @@ sixel_emit1b_kernel(typename A::Params G, SixelWork W) {
         const uint32_t done = head + 4u * nw;
         for (uint32_t k = done; k < local; ++k) d[k] = (char)(slot[(k >> 2) * ET] >> (8u * (k & 3u)));
     };
-    // emit5: the entry array is dead (every walk ended before the scan's barriers) and holds the band's image when no
-    // slot overflowed (<= 84 bytes a thread) and the image fits its 24*w bytes (narrow bands)
-    if (V5 && !__syncthreads_or(ovf) && band_total <= 24u * (uint32_t)w) {
+    // the entry array is dead (every walk ended before the scan's barriers) and holds the band's image when no slot
+    // overflowed (<= 84 bytes a thread) and the image fits its 24*w bytes (narrow bands)
+    if (!__syncthreads_or(ovf) && band_total <= 24u * (uint32_t)w) {
         char *img = reinterpret_cast<char *>(s_sorted);
         slot_out(img + at);
         __syncthreads();
@@ -1056,7 +792,7 @@ sixel_emit1b_kernel(typename A::Params G, SixelWork W) {
         if (t < band_total) band_out[t] = img[t];
     } else if (!ovf) {
         slot_out(o);
-    } else {                                                 // v1's write walk for this thread's range
+    } else {                                                 // slot overflow: this thread's range byte by byte
         walk_runs(s_sorted, lo, hi, n, [&](uint32_t c, uint32_t bits, uint32_t gap, uint32_t len, bool first) {
             if (first) { if (c != minc) *o++ = '$'; *o++ = '#'; o = put_num4(o, c); }
             o = put_rle(o, gap, '?');
@@ -1064,7 +800,7 @@ sixel_emit1b_kernel(typename A::Params G, SixelWork W) {
         });
     }
     EMIT_CLK();                                              // copy-out
-    EMIT_CLK_END(V5 ? 1 : 0);
+    EMIT_CLK_END();
 }
 
 // per frame: header length, band offsets (exclusive, in place), frame size
@@ -1204,8 +940,7 @@ static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 // slice with the scaler of the next.
 struct SixelPlan {
     SixelWork W;
-    bool emit_v1, dither_v1;
-    int emit_mode;                            // 1: v1, 4: v1b, 5: emit5 (scratch arena + compaction), 2: emit2, 3: emit3
+    int emit_mode;                            // 5: emit5 (scratch arena + compaction), 2: emit2
     EmitGeom G;
     SixelPaletteShape pal;
     size_t emit_smem, o_d2_bnd, o_d2_prog;
@@ -1236,17 +971,15 @@ SixelPaletteShape sixel_palette_shape(long long npix) {
     return P;
 }
 
-// The emitters (B200TIMG_EMIT=1..5): v1, v1b (4) and emit5 (5, the default up to 4095 px) write per-band bytes into a
-// scratch arena for the compaction kernel; emit2 (sixel_emit.cu: single pass, any width -- what wider frames get) and
-// emit3 (v1's sort + entry-parallel formatting + look-back placement; slower than v1 on C2 frames) place their own.
-// Every mode but the default is kept for A/B runs.
+// The emitters: emit5 (5, frames up to 4095 px) writes per-band bytes into a scratch arena for the compaction kernel;
+// emit2 (2, sixel_emit.cu: single pass, any width -- what wider frames get) places its own.  B200TIMG_EMIT=2 forces emit2
+// at any width, so that tests can run it on narrow frames (so does any value but 5; =5 stays emit2 above 4095 px).
 int sixel_emit_mode(int w) {
-    const bool v1_fits = w <= 4095 && sizeof(uint32_t) * (size_t)6 * w <= (size_t)(227 - 36) * 1024;
-    const bool v1b_fits = w <= 4095 && sizeof(uint32_t) * (size_t)6 * w <= (size_t)(227 - 47) * 1024;
-    int mode = v1b_fits ? 5 : v1_fits ? 1 : 2;           // 5 = emit5 (v1b with staged rows and a coalesced copy-out)
-    if (getenv("B200TIMG_EMIT_V2")) mode = 2;
+    // emit5's entry array (6*w words of dynamic shared memory) next to its ~47 KB of static shared memory
+    const bool emit5_fits = w <= 4095 && sizeof(uint32_t) * (size_t)6 * w <= (size_t)(227 - 47) * 1024;
+    int mode = emit5_fits ? 5 : 2;
     if (const char *e = getenv("B200TIMG_EMIT")) mode = atoi(e);
-    if (mode < 1 || mode > 5 || (mode == 1 && !v1_fits) || (mode >= 4 && !v1b_fits)) mode = 2;
+    if (mode != 5 || !emit5_fits) mode = 2;
     return mode;
 }
 
@@ -1273,9 +1006,7 @@ static int sixel_plan(b200timg_ctx *ctx, int w, int h, int n_frames, bool reserv
     W.band_cap = align_up((size_t)w * 42 + 256 * 5 + 16, 256);
     const size_t o_scr = off;
     S->emit_mode = sixel_emit_mode(w);
-    S->emit_v1 = S->emit_mode == 1 || S->emit_mode >= 4;
-    if (S->emit_v1) off += W.band_cap * W.nbands * n_frames;
-    S->dither_v1 = getenv("B200TIMG_DITHER_V1") != nullptr;      // round-1 ditherer, kept for A/B runs
+    if (S->emit_mode == 5) off += W.band_cap * W.nbands * n_frames;
     size_t d_bnd, d_prog;
     const size_t o_d2 = off; off += sixel_dither_workspace(w, h, n_frames, &d_bnd, &d_prog);
     size_t e_hdr, e_desc, e_ctl;
@@ -1294,14 +1025,10 @@ static int sixel_plan(b200timg_ctx *ctx, int w, int h, int n_frames, bool reserv
     W.ctl = reinterpret_cast<uint32_t *>(base + o_e2 + e_ctl);
     S->o_d2_bnd = o_d2 + d_bnd; S->o_d2_prog = o_d2 + d_prog;
     S->G.w = w; S->G.h = h; S->G.cols_per_warp = ((w + EW - 1) / EW + 31) / 32 * 32;
-    const size_t smem_limit = 227 * 1024 - 36 * 1024;   // the emit kernel also has ~33 KB of static shared memory
     S->emit_smem = sizeof(uint32_t) * (size_t)6 * w;
     if (!ctx->sixel_attrs_set) {                         // function attributes are per device, i.e. per context
         B2_CUDA(ctx, cudaFuncSetAttribute(sixel_palette_kernel<false, PaletteUniform>, cudaFuncAttributeMaxDynamicSharedMemorySize, 65536));
-        B2_CUDA(ctx, cudaFuncSetAttribute(sixel_emit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit));
-        B2_CUDA(ctx, cudaFuncSetAttribute(sixel_emit1b_kernel<false, EmitBands>, cudaFuncAttributeMaxDynamicSharedMemorySize, (227 - 47) * 1024));
-        B2_CUDA(ctx, cudaFuncSetAttribute(sixel_emit1b_kernel<true, EmitBands>, cudaFuncAttributeMaxDynamicSharedMemorySize, (227 - 47) * 1024));
-        B2_CUDA(ctx, cudaFuncSetAttribute(sixel_dither_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 32768 + DW_MAX * DWARP_SMEM));
+        B2_CUDA(ctx, cudaFuncSetAttribute(sixel_emit5_kernel<EmitBands>, cudaFuncAttributeMaxDynamicSharedMemorySize, (227 - 47) * 1024));
         // unconditionally: which variant a frame takes depends on ITS size, not on the first frame this context saw
         B2_CUDA(ctx, cudaFuncSetAttribute(sixel_palette_kernel<true, PaletteUniform>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
         ctx->sixel_attrs_set = true;
@@ -1309,7 +1036,7 @@ static int sixel_plan(b200timg_ctx *ctx, int w, int h, int n_frames, bool reserv
     return B200TIMG_OK;
 }
 
-// frames [f0, f0 + n) of a batch of n_total: palette -> table -> (map | dither) -> band sizes (v1 emitter), on ctx->stream
+// frames [f0, f0 + n) of a batch of n_total: palette -> table -> (map | dither) -> band bytes (emit5), on ctx->stream
 int launch_sixel_front(b200timg_ctx *ctx, const uint8_t *d_fb, int w, int h, int n_total, int f0, int n, bool reserve) {
     if ((reinterpret_cast<uintptr_t>(d_fb) & 3)) return ctx->fail(B200TIMG_EINVAL, "sixel: framebuffer must be 4-byte aligned");
     SixelPlan S;
@@ -1335,23 +1062,11 @@ int launch_sixel_front(b200timg_ctx *ctx, const uint8_t *d_fb, int w, int h, int
         sixel_map_kernel<MapUniform><<<dim3((unsigned)blocks, n), 256, 0, ctx->stream>>>(fb, npix, W, NoMixed());
         B2_LAUNCH_CHECK(ctx);
     }
-    if (!S.dither_v1) {
-        B2_TRY(launch_sixel_dither(ctx, fb, w, h, n, n_total, W, base + S.o_d2_bnd + sizeof(uint4) * (size_t)f0 * W.nb32 * w,
-                                   base + S.o_d2_prog + sizeof(int) * (size_t)f0 * W.nb32));
-    } else {
-        B2_KERNEL(ctx, "sixel_dither_kernel");
-        // warps per frame: as many as fit, but in full rounds over the 32-row bands
-        const int rounds = (W.nb32 + DW_MAX - 1) / DW_MAX;
-        const int nwarps = (W.nb32 + rounds - 1) / rounds;
-        const size_t dsmem = 32768 + (size_t)nwarps * DWARP_SMEM;
-        sixel_dither_kernel<<<n, nwarps * 32, dsmem, ctx->stream>>>(fb, w, h, nwarps, W);
-        B2_LAUNCH_CHECK(ctx);
-    }
-    if (S.emit_v1) {
-        B2_KERNEL(ctx, S.emit_mode == 5 ? "sixel_emit5_kernel" : "sixel_emit_kernel");
-        if (S.emit_mode == 5) sixel_emit1b_kernel<true, EmitBands><<<dim3(W.nbands, n), ET, S.emit_smem, ctx->stream>>>(S.G, W);
-        else if (S.emit_mode == 4) sixel_emit1b_kernel<false, EmitBands><<<dim3(W.nbands, n), ET, S.emit_smem, ctx->stream>>>(S.G, W);
-        else sixel_emit_kernel<<<dim3(W.nbands, n), ET, S.emit_smem, ctx->stream>>>(S.G, W);
+    B2_TRY(launch_sixel_dither(ctx, fb, w, h, n, n_total, W, base + S.o_d2_bnd + sizeof(uint4) * (size_t)f0 * W.nb32 * w,
+                               base + S.o_d2_prog + sizeof(int) * (size_t)f0 * W.nb32));
+    if (S.emit_mode == 5) {
+        B2_KERNEL(ctx, "sixel_emit5_kernel");
+        sixel_emit5_kernel<EmitBands><<<dim3(W.nbands, n), ET, S.emit_smem, ctx->stream>>>(S.G, W);
         B2_LAUNCH_CHECK(ctx);
     }
     return B200TIMG_OK;
@@ -1362,10 +1077,9 @@ int launch_sixel_back(b200timg_ctx *ctx, int w, int h, int n_frames, char *d_out
     SixelPlan S;
     B2_TRY(sixel_plan(ctx, w, h, n_frames, false, &S));
     const SixelWork &W = S.W;
-    if (!S.emit_v1) {
+    if (S.emit_mode == 2) {
         if (!(phases & 2)) return B200TIMG_OK;
-        if (S.emit_mode == 2) return launch_sixel_emit(ctx, w, h, n_frames, W, d_out, out_cap, d_offsets);
-        return launch_sixel_emit3(ctx, w, h, n_frames, W, d_out, out_cap, d_offsets);
+        return launch_sixel_emit(ctx, w, h, n_frames, W, d_out, out_cap, d_offsets);
     }
     if (phases & 1) {
         B2_KERNEL(ctx, "sixel_layout_kernel");
@@ -1491,7 +1205,7 @@ int launch_sixel_mixed(b200timg_ctx *ctx, const MixedPlan &mp, const char *d_are
     M.n_frames = n; M.nwarps = mp.sixel_nwarps;
     B2_CUDA(ctx, cudaFuncSetAttribute(sixel_palette_kernel<true, PaletteMixed>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     B2_CUDA(ctx, cudaFuncSetAttribute(sixel_palette_kernel<false, PaletteMixed>, cudaFuncAttributeMaxDynamicSharedMemorySize, 65536));
-    B2_CUDA(ctx, cudaFuncSetAttribute(sixel_emit1b_kernel<true, BandMixed>, cudaFuncAttributeMaxDynamicSharedMemorySize, (227 - 47) * 1024));
+    B2_CUDA(ctx, cudaFuncSetAttribute(sixel_emit5_kernel<BandMixed>, cudaFuncAttributeMaxDynamicSharedMemorySize, (227 - 47) * 1024));
     for (int k = 0; k < 2; ++k) {                 // every launch runs even without frames: the launch count stays fixed
         M.list = reinterpret_cast<const int *>(d_arena + mp.o_slist[k]);
         M.n_list = mp.sixel_list[k];
@@ -1510,7 +1224,7 @@ int launch_sixel_mixed(b200timg_ctx *ctx, const MixedPlan &mp, const char *d_are
     B2_LAUNCH_CHECK(ctx);
     B2_TRY(launch_sixel_dither_mixed(ctx, fb, mp.sixel_ctas, M, W, base + o_bnd, base + o_prog, mp.sixel_prog, mp.sixel_split != 0));
     B2_KERNEL(ctx, "sixel_emit5_mixed_kernel");
-    sixel_emit1b_kernel<true, BandMixed><<<mp.sixel_bands, ET, sizeof(uint32_t) * (size_t)6 * mp.sixel_wmax, ctx->stream>>>(M, W);
+    sixel_emit5_kernel<BandMixed><<<mp.sixel_bands, ET, sizeof(uint32_t) * (size_t)6 * mp.sixel_wmax, ctx->stream>>>(M, W);
     B2_LAUNCH_CHECK(ctx);
     B2_KERNEL(ctx, "sixel_layout_mixed_kernel");
     sixel_layout_kernel<LayoutMixed><<<n, 256, 0, ctx->stream>>>(0, 0, W, M);
@@ -1557,10 +1271,10 @@ extern "C" int b200timg_sixel_shape_of(int w, int h, int n_frames, int n_total, 
 }
 
 #ifdef B200TIMG_EMIT_CLOCKS
-// instrumented builds only: the summed phase clocks [2][8] since the last call (then cleared); 0 or -3 (CUDA error)
+// instrumented builds only: emit5's summed phase clocks [8] since the last call (then cleared); 0 or -3 (CUDA error)
 extern "C" int b200timg_emit_clocks(unsigned long long *out) {
     using b200timg::g_emit_clocks;
-    static const unsigned long long zero[2][b200timg::EMIT_CLK_PHASES] = {};
+    static const unsigned long long zero[b200timg::EMIT_CLK_PHASES] = {};
     if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpyFromSymbol(out, g_emit_clocks, sizeof zero) != cudaSuccess ||
         cudaMemcpyToSymbol(g_emit_clocks, zero, sizeof zero) != cudaSuccess)
         return -3;

@@ -116,8 +116,6 @@ __device__ __forceinline__ uint32_t column_entries(const uint8_t *__restrict__ i
 
 int launch_sixel_emit(b200timg_ctx *ctx, int w, int h, int n_frames, const SixelWork &W, char *d_out, size_t out_cap,
                       uint64_t *d_offsets);
-int launch_sixel_emit3(b200timg_ctx *ctx, int w, int h, int n_frames, const SixelWork &W, char *d_out, size_t out_cap,
-                       uint64_t *d_offsets);
 size_t sixel_dither_workspace(int w, int h, int n_frames, size_t *o_bnd, size_t *o_prog);
 int launch_sixel_dither(b200timg_ctx *ctx, const uint32_t *fb, int w, int h, int n_frames, int n_total, const SixelWork &W, void *d_bnd, void *d_prog);
 
@@ -136,8 +134,8 @@ SixelPaletteShape sixel_palette_shape(long long npix);
 // band above).  env: honour B200TIMG_DITHER_SPLIT / B200TIMG_DITHER_WARPS (the uniform launches do, mixed batches do not).
 struct SixelDitherShape { int per_frame, bands_per_cta, nwarps, rounds; };
 SixelDitherShape sixel_dither_shape(int nb32, int n_frames, int n_total, int sm_count, bool env);
-// K6: the emitter a frame w wide takes (1 v1, 4 v1b, 5 emit5: band scratch + compaction; 2 emit2, 3 emit3: single pass;
-// B200TIMG_EMIT / B200TIMG_EMIT_V2 honoured) and the single-pass emitters' column tiles.
+// K6: the emitter a frame w wide takes (5 emit5: band scratch + compaction; 2 emit2: single pass; B200TIMG_EMIT honoured)
+// and emit2's column tiles.
 int sixel_emit_mode(int w);
 void sixel_emit_tiling(int w, int *ntiles, int *tw, int *cpw);
 

@@ -9,11 +9,11 @@ interleaved, round after round, so every mode is measured under the same conditi
 are read in the same run.
 
 --clocks also compiles sixel.cu with -DB200TIMG_EMIT_CLOCKS into a temporary directory, links it with the tree's other
-objects (left there by the regular build) and reports, per mode with an instrumented kernel (4: emit1b, 5: emit5), the
-share of each phase in the SM cycles its CTAs spent (the instrumented build adds CTA barriers at the phase boundaries,
-so its kernel times are not the product's).
+objects (left there by the regular build) and reports, for mode 5 (emit5, the instrumented kernel), the share of each
+phase in the SM cycles its CTAs spent (the instrumented build adds CTA barriers at the phase boundaries, so its kernel
+times are not the product's).
 
-    python tools/bench_sixel_emit.py [--configs C2,C5] [--modes 4,5] [--rounds 2] [--steps 5] [--warmup 2] [--clocks]
+    python tools/bench_sixel_emit.py [--configs C2,C5] [--modes 5,2] [--rounds 2] [--steps 5] [--warmup 2] [--clocks]
 
 Prints one JSON line per (round, config, mode), a first line describing the card, and with --clocks one line per
 (config, mode) of phase shares.  Writes nothing to the tree.
@@ -35,10 +35,8 @@ import bench  # noqa: E402  (CONFIGS, frames_torch: the flagship's geometries an
 SRC = os.path.join(ROOT, "timg_b200", "csrc")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
-# the phases each instrumented kernel stamps, in order (sixel.cu EMIT_CLK)
-PHASES = {4: ["zero", "count", "offsets", "scatter", "walk", "scan", "copy-out"],
-          5: ["zero+count", "offsets", "scatter", "walk", "scan", "copy-out"]}
-CLK_ROW = {4: 0, 5: 1}
+# the phases emit5 stamps, in order (sixel.cu EMIT_CLK)
+PHASES = ["zero+count", "offsets", "scatter", "walk", "scan", "copy-out"]
 EMIT_KEYS = ("emit", "layout", "offsets", "compact")
 
 
@@ -76,7 +74,7 @@ def build_instrumented(tmp):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--configs", default="C2,C5")
-    ap.add_argument("--modes", default="4,5")
+    ap.add_argument("--modes", default="5,2")
     ap.add_argument("--rounds", type=int, default=2)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
@@ -98,7 +96,7 @@ def main():
             finally:
                 shutil.rmtree(tmp, ignore_errors=True)
         return
-    run(args, [m for m in modes if m in PHASES], clocks=True)
+    run(args, [m for m in modes if m == 5], clocks=True)
 
 
 def run(args, modes, clocks):
@@ -145,17 +143,17 @@ def run(args, modes, clocks):
                     step(b, src, out, offs, cap)
                 torch.cuda.synchronize(dev)
                 if clocks:
-                    raw = (C.c_ulonglong * 16)()
+                    raw = (C.c_ulonglong * 8)()
                     get_clocks(raw)
                     for _ in range(args.steps):
                         step(b, src, out, offs, cap)
                     if get_clocks(raw) != 0:
                         raise RuntimeError("b200timg_emit_clocks failed")
-                    row = [raw[CLK_ROW[mode] * 8 + k] for k in range(len(PHASES[mode]))]
+                    row = [raw[k] for k in range(len(PHASES))]
                     tot = sum(row) or 1
                     print(json.dumps({"clocks": True, "config": cname, "mode": mode, "bands": n * hp // 6,
                                       "sm_cycles_per_band": tot / (args.steps * n * hp // 6),
-                                      "share": {p: round(v / tot, 4) for p, v in zip(PHASES[mode], row)}}), flush=True)
+                                      "share": {p: round(v / tot, 4) for p, v in zip(PHASES, row)}}), flush=True)
                     continue
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 e0.record(stream)
