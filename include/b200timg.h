@@ -354,6 +354,52 @@ typedef struct {
 } b200timg_sixel_shape;
 int b200timg_sixel_shape_of(int w, int h, int n_frames, int n_total, int sm_count, b200timg_sixel_shape *out);
 
+/* Host-only introspection of the scaler's launch shape (no GPU needed): the route, tap classes and windows the bit-exact
+ * (fast == 0) or FAST (fast == 1) scale of n_frames frames of iw x ih -> ow x oh takes, with the source (src_aligned16)
+ * and output (dst_aligned16) pointers 16-byte aligned or not.  Computed by the function launch_scale calls, the
+ * environment switches it honours included (B200TIMG_NO_PLANAR, B200TIMG_NO_H1S, B200TIMG_NO_H1F, B200TIMG_TMA).
+ * Routes, in the order they are tried:
+ *   COPY4   both axes point-sampled onto themselves, ow % 4 == 0, both pointers aligned: 16-byte copy
+ *   COPY    both axes point-sampled otherwise: resample_copy_kernel
+ *   V3      FAST only, where PLANAR fits and v3_smem <= 100 KB and 32 * 65 <= the window's words: opaque 64 x 32 tiles in
+ *           resample_v3_kernel<hc,vc>, tiles with transparency in resample_planar_list_kernel<hc,vc>
+ *   PLANAR  vertical pass first, <= 8 taps per axis, iw % 4 == 0, aligned source, planar_smem <= 75 KB and
+ *           32 * 33 <= 3 * the window's words: 32 x 32 tiles of resample_planar_kernel<hc,vc>
+ *   FIXED   <= 8 taps per axis, fixed_smem <= 100 KB: 64 x 16 tiles of resample_fixed_kernel<vertical_first,hc,vc>
+ *   TP_V    the two 1-D passes, vertical first (twopass_v1 + twopass_2)
+ *   TP_H1S / TP_H1F / TP_H1   the two passes, horizontal first; the first pass is the staged one where h1s_smem <= 72 KB
+ *           and the 32-column tiles are mostly full (ceil(ow / 32) * 32 <= 1.15 * ow), the flat (row, column) one for
+ *           other widths up to ow = 4096 (h1f_rows rows per CTA), else the plain tiled one.
+ *   Every two-pass route runs a second, plain pair of passes for outputs whose filtered alpha is below 2^-120.
+ * hc / vc: taps per axis rounded up to 2, 4, 6 or 8 (0 above 8 taps).  The smem fields hold the shared-memory bytes of
+ * each candidate the decision evaluated (0 when it did not get there); tiles_x / tiles_y and win_w / win_h: the chosen
+ * kernel's tile grid and the source window of its widest tile (two-pass routes: the second pass's 32 x 8 grid, no
+ * window).  Returns B200TIMG_EINVAL for a degenerate geometry, out == NULL, n_frames <= 0, and more than 65535 frames
+ * on any route but the copies. */
+#define B200TIMG_SCALE_COPY4   1
+#define B200TIMG_SCALE_COPY    2
+#define B200TIMG_SCALE_V3      3
+#define B200TIMG_SCALE_PLANAR  4
+#define B200TIMG_SCALE_FIXED   5
+#define B200TIMG_SCALE_TP_V    6
+#define B200TIMG_SCALE_TP_H1S  7
+#define B200TIMG_SCALE_TP_H1F  8
+#define B200TIMG_SCALE_TP_H1   9
+typedef struct {
+    int route;                                 /* B200TIMG_SCALE_* */
+    int hc, vc, h_widest, v_widest;            /* tap classes and the plan's widest tap counts */
+    int vertical_first, h_sequential;          /* pass order; horizontal taps on one accumulator (widest <= 3) */
+    int h_filter, v_filter, h_gather, v_gather;/* per axis: 0 point, 1 box, 2 Mitchell; 1 enlarging gather, 2 shrinking
+                                                  gather, 0 scatter */
+    int h1f_rows;                              /* TP_H1F: rows per CTA, else 0 */
+    int v3_tma;                                /* V3: the window qualifies for TMA staging (sp <= 256 columns, <= 256 rows) */
+    int planar_reuse, v3_reuse, tiles_full;    /* the reuse rules of PLANAR and V3, the 115 % rule of TP_H1S */
+    int planar_smem, v3_smem, fixed_smem, h1s_smem;
+    int tiles_x, tiles_y, win_w, win_h;
+} b200timg_scale_shape;
+int b200timg_scale_shape_of(int iw, int ih, int ow, int oh, int n_frames, int fast, int src_aligned16, int dst_aligned16,
+                            b200timg_scale_shape *out);
+
 /* ======================= geometry passes around the path (SURVEY 8f rank 3, row a15) ===============
  * ApplyExifOp (src/jpeg-source.cc:84-119): mirror each row, then rotate by 0, 180, 90 or -90 degrees exactly as
  * the reference's loops do (90 / -90: out is h x w).  in and out: w*h*4 bytes. */

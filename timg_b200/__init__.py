@@ -66,6 +66,16 @@ class SixelShape(C.Structure):
                                        "dither_warps", "dither_rounds", "emit_mode", "emit_tiles", "tile_w")]
 
 
+SCALE_ROUTES = {1: "copy4", 2: "copy", 3: "v3", 4: "planar", 5: "fixed", 6: "tp_v", 7: "tp_h1s", 8: "tp_h1f", 9: "tp_h1"}
+
+
+class ScaleShape(C.Structure):
+    _fields_ = [(k, C.c_int) for k in ("route", "hc", "vc", "h_widest", "v_widest", "vertical_first", "h_sequential", "h_filter",
+                                       "v_filter", "h_gather", "v_gather", "h1f_rows", "v3_tma", "planar_reuse", "v3_reuse",
+                                       "tiles_full", "planar_smem", "v3_smem", "fixed_smem", "h1s_smem", "tiles_x", "tiles_y",
+                                       "win_w", "win_h")]
+
+
 class MixedBatch(C.Structure):
     _fields_ = [("n_frames", C.c_int), ("src_fmt", C.c_int), ("flags", C.c_int), ("has_bg", C.c_int), ("bg", C.c_uint32),
                 ("pattern", C.c_uint32), ("pattern_w", C.c_int), ("pattern_h", C.c_int), ("frames", C.POINTER(Frame))]
@@ -143,6 +153,7 @@ ABI = {
     "b200timg_resample_plan": (C.c_int, [C.c_int] * 5 + [C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p,
                                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     "b200timg_sixel_shape_of": (C.c_int, [C.c_int] * 5 + [C.POINTER(SixelShape)]),
+    "b200timg_scale_shape_of": (C.c_int, [C.c_int] * 8 + [C.POINTER(ScaleShape)]),
 }
 
 _lib = None
@@ -216,6 +227,18 @@ def sixel_shape(w, h, n_frames=1, n_total=None, sm_count=132):
     if rc != OK:
         raise B200Error(rc, f"sixel_shape: {w} x {h}, {n_frames} frames: not a geometry the sixel path takes")
     return {k: getattr(s, k) for k, _ in SixelShape._fields_}
+
+
+def scale_shape(iw, ih, ow, oh, n_frames=1, fast=False, src_aligned16=True, dst_aligned16=True):
+    """Host-side launch shape of the scaler for n_frames frames of iw x ih -> ow x oh, as a dict of b200timg_scale_shape's
+    fields (see include/b200timg.h) with the route's name under "route"."""
+    s = ScaleShape()
+    rc = lib().b200timg_scale_shape_of(iw, ih, ow, oh, n_frames, int(bool(fast)), int(src_aligned16), int(dst_aligned16), C.byref(s))
+    if rc != OK:
+        raise B200Error(rc, f"scale_shape: {iw} x {ih} -> {ow} x {oh}, {n_frames} frames: not a geometry the scaler takes")
+    d = {k: getattr(s, k) for k, _ in ScaleShape._fields_}
+    d["route"] = SCALE_ROUTES[d["route"]]
+    return d
 
 
 def graphics(protocol, rgb24=False, ids=None, cell=None, indent=0):

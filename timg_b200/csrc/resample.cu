@@ -1073,6 +1073,22 @@ static bool v3_tensor_map(CUtensorMap *map, const uint32_t *src, int iw, int ih,
 #endif
 }
 
+// the host-side part of v3_tensor_map's conditions: a window of box_cols x box_rows words at a 16-byte row pitch
+static bool v3_tma_eligible(int iw, bool src16, int box_cols, int box_rows) {
+#ifdef CUSIM
+    return false;
+#else
+    if (const char *e = getenv("B200TIMG_TMA")) if (atoi(e) == 0) return false;
+    return (iw & 3) == 0 && src16 && box_cols <= 256 && box_rows <= 256 && (box_cols & 3) == 0;
+#endif
+}
+
+// dynamic shared memory caps of the scaler's kernels (what the launch selection compares against)
+constexpr size_t PLANAR_SMEM_CAP = 75 * 1024;    // 3 CTAs/SM (80 registers) rather than 2
+constexpr size_t V3_SMEM_CAP = 100 * 1024;
+constexpr size_t FIXED_SMEM_CAP = 100 * 1024;
+constexpr size_t H1S_SMEM_CAP = 72 * 1024;
+
 typedef void (*V3Fn)(const uint32_t *, uint32_t *, ResampleParams, V3Geom, const CUtensorMap);
 template <int HC>
 static V3Fn v3_v(int vc) {
@@ -1108,6 +1124,122 @@ static PlanarListFn planar_list_h(int hc, int vc) {
     case 6: return planar_list_v<6>(vc);
     default: return planar_list_v<8>(vc);
     }
+}
+
+// ---- launch shape ------------------------------------------------------------------------------------------------
+// Route, tap classes, windows and tile origins of one scale call, from the plan, the geometry and the pointers'
+// alignment.  launch_scale launches what this returns and b200timg_scale_shape_of reports it.  all = evaluate every
+// candidate whose tap counts allow it (the introspection), not only those the decision reaches.
+struct ScaleShape {
+    int route = 0, hc = 0, vc = 0;
+    bool planar_reuse = false, v3_reuse = false, tiles_full = false, v3_tma = false;
+    size_t psmem = 0, v3smem = 0, fsmem = 0, h1smem = 0;
+    int nix = 0, niy = 0, sp = 0, tp = 0, nix3 = 0, sp3 = 0, tp3 = 0;   // planar / v3 windows and pitches
+    std::vector<int32_t> tix, tiy, tix3;                                // their tile origins
+    FixedVariant fv{};
+    int fnix = 0, fniy = 0;
+    std::vector<int32_t> ftix, ftiy;                                    // fixed kernel: window and tile origins
+    H1sGeom hg{1, 1};
+    int h1f_rows = 0;
+};
+
+static ScaleShape scale_shape(const ResamplePlan &pl, int iw, int ih, int ow, int oh, int n_frames, bool fast, bool src16,
+                              bool dst16, bool all) {
+    ScaleShape S;
+    bool identity = pl.copy_only && iw == ow && ih == oh && (ow & 3) == 0 && n_frames <= 65535 && (long long)ow * oh < (1ll << 31) &&
+                    src16 && dst16;
+    for (int x = 0; identity && x < ow; ++x) identity = pl.h.first[x] == x;
+    for (int y = 0; identity && y < oh; ++y) identity = pl.v.first[y] == y;
+    if (identity) { S.route = B200TIMG_SCALE_COPY4; return S; }
+    if (pl.copy_only) { S.route = B200TIMG_SCALE_COPY; return S; }
+    const bool small = pl.h.widest <= 8 && pl.v.widest <= 8;
+    if (small) { S.hc = fixed_class(pl.h.widest); S.vc = fixed_class(pl.v.widest); }
+    // fastest path: vertical pass first, <= 8 taps per axis, 16-byte aligned rows -> v3 kernel (opaque tiles)
+    // with the planar kernel taking the tiles that contain transparency
+    const bool planar_gate = pl.vertical_first && small && (iw & 3) == 0 && src16 && !getenv("B200TIMG_NO_PLANAR");
+    if (small && (planar_gate || all)) {
+        auto tile_origins = [&](const AxisTable &T, int n_out, int tile, int taps, bool align4, std::vector<int32_t> &orig) -> int {
+            const int nt = (n_out + tile - 1) / tile;
+            orig.resize(nt);
+            int span = 1;
+            for (int j = 0; j < nt; ++j) {
+                int lo = 0x7fffffff, hi = -1;
+                for (int x = j * tile; x < std::min(n_out, (j + 1) * tile); ++x) { lo = std::min(lo, T.first[x]); hi = std::max(hi, T.first[x] + taps - 1); }
+                if (align4) lo &= ~3;                            // aligned 16-byte loads
+                orig[j] = lo; span = std::max(span, hi - lo + 1);
+            }
+            return span;
+        };
+        const int ptw = 32;
+        S.nix = tile_origins(pl.h, ow, ptw, S.hc, true, S.tix); S.niy = tile_origins(pl.v, oh, PTH, S.vc, false, S.tiy);
+        S.sp = (S.nix + 3) & ~3; S.tp = S.sp | 1;   // odd T pitch >= the 4-column groups written per row
+        S.psmem = sizeof(float) * (3 * ((size_t)S.niy * S.sp + (size_t)PTH * S.tp) + 4 + (size_t)ptw * 8 + PTH * 8) + sizeof(int) * (ptw + PTH);
+        S.planar_reuse = (size_t)PTH * (ptw + 1) <= 3 * (size_t)S.niy * S.sp;
+        const bool planar_ok = S.psmem <= PLANAR_SMEM_CAP && S.planar_reuse;   // 3 CTAs/SM (80 registers) rather than 2
+        // v3 geometry: 64 x 32 output tiles
+        S.nix3 = tile_origins(pl.h, ow, V3_TW, S.hc, true, S.tix3);
+        S.sp3 = (S.nix3 + 3) & ~3; S.tp3 = S.sp3 | 1;
+        S.v3smem = sizeof(uint32_t) * (size_t)S.niy * S.sp3 + (sizeof(float2) + sizeof(float)) * (size_t)V3_TH * S.tp3 + 16 +
+                   sizeof(float) * ((size_t)V3_TW * 8 + V3_TH * 8) + sizeof(int) * (V3_TW + V3_TH + 2);
+        S.v3_reuse = (size_t)V3_TH * (V3_TW + 1) <= (size_t)S.niy * S.sp3;
+        // v3 pays off in the FAST arithmetic only; bit-exact scaling takes the planar kernel
+        const bool v3_ok = planar_ok && fast && S.v3smem <= V3_SMEM_CAP && S.v3_reuse;
+        S.v3_tma = v3_tma_eligible(iw, src16, S.sp3, S.niy);
+        if (planar_gate && planar_ok) S.route = v3_ok ? B200TIMG_SCALE_V3 : B200TIMG_SCALE_PLANAR;
+    }
+    if (small && (!S.route || all)) {
+        S.fv = pl.vertical_first ? fixed_h<true>(S.hc, S.vc) : fixed_h<false>(S.hc, S.vc);
+        const int FTHv = S.fv.th;
+        const int ntx = (ow + FTW - 1) / FTW, nty = (oh + FTHv - 1) / FTHv;
+        S.ftix.resize(ntx); S.ftiy.resize(nty);
+        S.fnix = 1; S.fniy = 1;
+        for (int j = 0; j < ntx; ++j) {
+            int lo = 0x7fffffff, hi = -1;
+            for (int x = j * FTW; x < std::min(ow, (j + 1) * FTW); ++x) { lo = std::min(lo, pl.h.first[x]); hi = std::max(hi, pl.h.first[x] + S.hc - 1); }
+            S.ftix[j] = lo; S.fnix = std::max(S.fnix, hi - lo + 1);
+        }
+        for (int j = 0; j < nty; ++j) {
+            int lo = 0x7fffffff, hi = -1;
+            for (int y = j * FTHv; y < std::min(oh, (j + 1) * FTHv); ++y) { lo = std::min(lo, pl.v.first[y]); hi = std::max(hi, pl.v.first[y] + S.vc - 1); }
+            S.ftiy[j] = lo; S.fniy = std::max(S.fniy, hi - lo + 1);
+        }
+        S.fsmem = sizeof(float4) * ((size_t)S.fnix * S.fniy + (pl.vertical_first ? (size_t)FTHv * S.fnix : (size_t)S.fniy * FTW))
+                + sizeof(int) * (FTW + FTHv) + sizeof(float) * ((size_t)FTW * (S.hc + 1) + (size_t)FTHv * (S.vc + 1));
+        if (!S.route && S.fsmem <= FIXED_SMEM_CAP) S.route = B200TIMG_SCALE_FIXED;
+    }
+    // long filters: two 1-D passes over a float4 intermediate in global memory
+    // staging pays when the 32-column tiles are mostly full (4K -> 337 columns); with 67 columns the third
+    // tile stages a whole window for 3 outputs: plain kernel
+    S.tiles_full = (long long)((ow + 31) / 32) * 32 * 100 <= (long long)ow * 115;
+    if (!pl.vertical_first || all) {
+        // staged variant: window of a 32-column tile = first[tile start] .. max(first + count) over the tile
+        S.hg = H1sGeom{1, pl.h.widest | 1};
+        for (int x0 = 0; x0 < ow; x0 += 32) {
+            int hi = 0;
+            for (int x = x0; x < std::min(ow, x0 + 32); ++x) hi = std::max(hi, pl.h.first[x] + pl.h.count[x]);
+            S.hg.nwin = std::max(S.hg.nwin, hi - pl.h.first[x0]);
+        }
+        S.h1smem = sizeof(float4) * 8 * (size_t)S.hg.nwin + sizeof(float) * 32 * (size_t)S.hg.cpitch;
+    }
+    if (S.route) return S;
+    if (pl.vertical_first) {
+        S.route = B200TIMG_SCALE_TP_V;
+    } else if (S.h1smem <= H1S_SMEM_CAP && S.tiles_full && !getenv("B200TIMG_NO_H1S")) {
+        S.route = B200TIMG_SCALE_TP_H1S;
+    } else if (!S.tiles_full && ow <= 4096 && n_frames <= 65535 && !getenv("B200TIMG_NO_H1F")) {
+        // few output columns: flat (row, column) mapping; rows per CTA chosen so that rows x ow fills whole 256-thread rounds
+        S.route = B200TIMG_SCALE_TP_H1F;
+        int rows = 8; double best = 0.0;
+        for (int r = 4; r <= 64; ++r) {
+            const long long items = (long long)r * ow, slots = (items + 255) / 256 * 256;
+            const double fill = (double)items / (double)slots;
+            if (fill > best + 1e-9) { best = fill; rows = r; }
+        }
+        S.h1f_rows = rows;
+    } else {
+        S.route = B200TIMG_SCALE_TP_H1;
+    }
+    return S;
 }
 
 // ---- plan cache + upload ----------------------------------------------------------------
@@ -1163,128 +1295,76 @@ int launch_scale(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int fmt
     P.v_coeff = reinterpret_cast<const float *>(t + o_vk);
     const uint32_t *in = reinterpret_cast<const uint32_t *>(d_in);
     uint32_t *out = reinterpret_cast<uint32_t *>(d_out);
-    bool identity = pl->copy_only && iw == ow && ih == oh && (ow & 3) == 0 && n_frames <= 65535 && (long long)ow * oh < (1ll << 31) &&
-                    ((reinterpret_cast<uintptr_t>(d_in) | reinterpret_cast<uintptr_t>(d_out)) & 15) == 0;
-    for (int x = 0; identity && x < ow; ++x) identity = pl->h.first[x] == x;
-    for (int y = 0; identity && y < oh; ++y) identity = pl->v.first[y] == y;
-    if (identity) {
+    const bool src16 = (reinterpret_cast<uintptr_t>(d_in) & 15) == 0, dst16 = (reinterpret_cast<uintptr_t>(d_out) & 15) == 0;
+    if (!pl->copy_only && n_frames > 65535) return ctx->fail(B200TIMG_EINVAL, "scale: too many frames for one launch");
+    ScaleShape S = scale_shape(*pl, iw, ih, ow, oh, n_frames, fast != 0, src16, dst16, false);
+    switch (S.route) {
+    case B200TIMG_SCALE_COPY4: {
         const int nq = (ow >> 2) * oh;
         const int bx = std::max(1, std::min((nq + 255) / 256, std::max(1, ctx->sm_count * 8 / std::max(1, std::min(n_frames, ctx->sm_count * 8)))));
         B2_KERNEL(ctx, "resample_copy_kernel");
         resample_copy4_kernel<<<dim3((unsigned)bx, (unsigned)n_frames), 256, 0, ctx->stream>>>(in, out, P);
-    } else if (pl->copy_only) {
+        break;
+    }
+    case B200TIMG_SCALE_COPY: {
         long long blocks = ((long long)ow * oh * n_frames + 255) / 256;
         if (blocks > (long long)ctx->sm_count * 16) blocks = (long long)ctx->sm_count * 16;
         B2_KERNEL(ctx, "resample_copy_kernel");
         resample_copy_kernel<<<(unsigned)blocks, 256, 0, ctx->stream>>>(in, out, P);
-    } else {
-        if (n_frames > 65535) return ctx->fail(B200TIMG_EINVAL, "scale: too many frames for one launch");
-        // fastest path: vertical pass first, <= 8 taps per axis, 16-byte aligned rows -> v3 kernel (opaque tiles)
-        // with the planar kernel taking the tiles that contain transparency
-        if (pl->vertical_first && pl->h.widest <= 8 && pl->v.widest <= 8 && (iw & 3) == 0 &&
-            (reinterpret_cast<uintptr_t>(d_in) & 15) == 0 && !getenv("B200TIMG_NO_PLANAR")) {
-            const int hc = fixed_class(pl->h.widest), vc = fixed_class(pl->v.widest);
-            auto tile_origins = [&](const AxisTable &T, int n_out, int tile, int taps, bool align4, std::vector<int32_t> &orig) -> int {
-                const int nt = (n_out + tile - 1) / tile;
-                orig.resize(nt);
-                int span = 1;
-                for (int j = 0; j < nt; ++j) {
-                    int lo = 0x7fffffff, hi = -1;
-                    for (int x = j * tile; x < std::min(n_out, (j + 1) * tile); ++x) { lo = std::min(lo, T.first[x]); hi = std::max(hi, T.first[x] + taps - 1); }
-                    if (align4) lo &= ~3;                            // aligned 16-byte loads
-                    orig[j] = lo; span = std::max(span, hi - lo + 1);
-                }
-                return span;
-            };
-            std::vector<int32_t> tix, tiy, tix3;
-            const int ptw = 32;
-            const int nix = tile_origins(pl->h, ow, ptw, hc, true, tix), niy = tile_origins(pl->v, oh, PTH, vc, false, tiy);
-            const int ntx = (int)tix.size(), nty = (int)tiy.size();
-            const int sp = (nix + 3) & ~3, tp = sp | 1;   // odd T pitch >= the 4-column groups written per row
-            const size_t psmem = sizeof(float) * (3 * ((size_t)niy * sp + (size_t)PTH * tp) + 4 + (size_t)ptw * 8 + PTH * 8) + sizeof(int) * (ptw + PTH);
-            const size_t smem_cap = 75 * 1024;           // 3 CTAs/SM (80 registers) rather than 2
-            const bool planar_ok = psmem <= smem_cap && (size_t)PTH * (ptw + 1) <= 3 * (size_t)niy * sp;
-            // v3 geometry: 64 x 32 output tiles
-            const int nix3 = tile_origins(pl->h, ow, V3_TW, hc, true, tix3);
-            const int ntx3 = (int)tix3.size();
-            const int sp3 = (nix3 + 3) & ~3, tp3 = sp3 | 1;
-            const size_t v3smem = sizeof(uint32_t) * (size_t)niy * sp3 + (sizeof(float2) + sizeof(float)) * (size_t)V3_TH * tp3 + 16 +
-                                  sizeof(float) * ((size_t)V3_TW * 8 + V3_TH * 8) + sizeof(int) * (V3_TW + V3_TH + 2);
-            // v3 pays off in the FAST arithmetic only; bit-exact scaling takes the planar kernel
-            const bool v3_ok = planar_ok && fast && v3smem <= 100 * 1024 &&
-                               (size_t)V3_TH * (V3_TW + 1) <= (size_t)niy * sp3;
-            if (planar_ok) {
-                B2_CUDA(ctx, ctx->misc.reserve(4096 + sizeof(int32_t) * (size_t)(ntx + nty + ntx3)));
-                int32_t *d_t = reinterpret_cast<int32_t *>(ctx->misc.as<char>() + 4096);
-                B2_CUDA(ctx, cudaMemcpyAsync(d_t, tix.data(), sizeof(int32_t) * ntx, cudaMemcpyHostToDevice, ctx->stream));
-                B2_CUDA(ctx, cudaMemcpyAsync(d_t + ntx, tiy.data(), sizeof(int32_t) * nty, cudaMemcpyHostToDevice, ctx->stream));
-                B2_CUDA(ctx, cudaMemcpyAsync(d_t + ntx + nty, tix3.data(), sizeof(int32_t) * ntx3, cudaMemcpyHostToDevice, ctx->stream));
-                PlanarGeom PG{nix, niy, sp, tp, (unsigned)(0x100000000ull / (unsigned)(sp / 4)) + 1u, d_t, d_t + ntx};
-                if (v3_ok) {
-                    // one work list per concurrently running slice of a batch (api.cu), sized before any slice starts
-                    const size_t list_words = 1 + 3 * (size_t)ntx3 * nty * (size_t)std::max(n_frames, ctx->part_max_frames);
-                    B2_CUDA(ctx, ctx->scale_list.reserve(sizeof(uint32_t) * list_words * (size_t)ctx->part_slots));
-                    uint32_t *d_list = ctx->scale_list.as<uint32_t>() + list_words * (size_t)ctx->part_slot;
-                    B2_CUDA(ctx, cudaMemsetAsync(d_list, 0, sizeof(uint32_t), ctx->stream));
-                    V3Geom VG{nix3, niy, sp3, tp3, (unsigned)(0x100000000ull / (unsigned)(sp3 / 4)) + 1u, d_t + ntx + nty, d_t + ntx, d_list, 0};
-                    CUtensorMap tmap;
-                    memset(&tmap, 0, sizeof tmap);
-                    VG.use_tma = v3_tensor_map(&tmap, in, iw, ih, n_frames, sp3, niy) ? 1 : 0;
-                    V3Fn fn = v3_h(hc, vc);
-                    B2_CUDA(ctx, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-                    B2_KERNEL(ctx, "resample_v3_fast_kernel");
-                    fn<<<dim3(ntx3, nty, n_frames), V3_NT, v3smem, ctx->stream>>>(in, out, P, VG, tmap);
-                    B2_LAUNCH_CHECK(ctx);
-                    PlanarListFn lf = planar_list_h(hc, vc);              // tiles with transparency (none for photos / video)
-                    B2_CUDA(ctx, cudaFuncSetAttribute(lf, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cap));
-                    B2_KERNEL(ctx, "resample_planar_list_kernel");
-                    lf<<<ctx->sm_count * 3, PNT, psmem, ctx->stream>>>(in, out, P, PG, d_list);
-                    B2_LAUNCH_CHECK(ctx);
-                    return B200TIMG_OK;
-                }
-                PlanarFn fn = planar_h<32, 3>(hc, vc);
-                B2_CUDA(ctx, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cap));
-                const dim3 grid(ntx, nty, n_frames);
-                B2_KERNEL(ctx, "resample_planar_kernel");
-                fn<<<grid, PNT, psmem, ctx->stream>>>(in, out, P, PG);
-                B2_LAUNCH_CHECK(ctx);
-                return B200TIMG_OK;
-            }
+        break;
+    }
+    case B200TIMG_SCALE_V3:
+    case B200TIMG_SCALE_PLANAR: {
+        const int ntx = (int)S.tix.size(), nty = (int)S.tiy.size(), ntx3 = (int)S.tix3.size();
+        B2_CUDA(ctx, ctx->misc.reserve(4096 + sizeof(int32_t) * (size_t)(ntx + nty + ntx3)));
+        int32_t *d_t = reinterpret_cast<int32_t *>(ctx->misc.as<char>() + 4096);
+        B2_CUDA(ctx, cudaMemcpyAsync(d_t, S.tix.data(), sizeof(int32_t) * ntx, cudaMemcpyHostToDevice, ctx->stream));
+        B2_CUDA(ctx, cudaMemcpyAsync(d_t + ntx, S.tiy.data(), sizeof(int32_t) * nty, cudaMemcpyHostToDevice, ctx->stream));
+        B2_CUDA(ctx, cudaMemcpyAsync(d_t + ntx + nty, S.tix3.data(), sizeof(int32_t) * ntx3, cudaMemcpyHostToDevice, ctx->stream));
+        PlanarGeom PG{S.nix, S.niy, S.sp, S.tp, (unsigned)(0x100000000ull / (unsigned)(S.sp / 4)) + 1u, d_t, d_t + ntx};
+        if (S.route == B200TIMG_SCALE_V3) {
+            // one work list per concurrently running slice of a batch (api.cu), sized before any slice starts
+            const size_t list_words = 1 + 3 * (size_t)ntx3 * nty * (size_t)std::max(n_frames, ctx->part_max_frames);
+            B2_CUDA(ctx, ctx->scale_list.reserve(sizeof(uint32_t) * list_words * (size_t)ctx->part_slots));
+            uint32_t *d_list = ctx->scale_list.as<uint32_t>() + list_words * (size_t)ctx->part_slot;
+            B2_CUDA(ctx, cudaMemsetAsync(d_list, 0, sizeof(uint32_t), ctx->stream));
+            V3Geom VG{S.nix3, S.niy, S.sp3, S.tp3, (unsigned)(0x100000000ull / (unsigned)(S.sp3 / 4)) + 1u, d_t + ntx + nty, d_t + ntx, d_list, 0};
+            CUtensorMap tmap;
+            memset(&tmap, 0, sizeof tmap);
+            VG.use_tma = S.v3_tma && v3_tensor_map(&tmap, in, iw, ih, n_frames, S.sp3, S.niy) ? 1 : 0;
+            V3Fn fn = v3_h(S.hc, S.vc);
+            B2_CUDA(ctx, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)V3_SMEM_CAP));
+            B2_KERNEL(ctx, "resample_v3_fast_kernel");
+            fn<<<dim3(ntx3, nty, n_frames), V3_NT, S.v3smem, ctx->stream>>>(in, out, P, VG, tmap);
+            B2_LAUNCH_CHECK(ctx);
+            PlanarListFn lf = planar_list_h(S.hc, S.vc);              // tiles with transparency (none for photos / video)
+            B2_CUDA(ctx, cudaFuncSetAttribute(lf, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PLANAR_SMEM_CAP));
+            B2_KERNEL(ctx, "resample_planar_list_kernel");
+            lf<<<ctx->sm_count * 3, PNT, S.psmem, ctx->stream>>>(in, out, P, PG, d_list);
+            break;
         }
-        if (pl->h.widest <= 8 && pl->v.widest <= 8) {
-            const int hc = fixed_class(pl->h.widest), vc = fixed_class(pl->v.widest);
-            const FixedVariant fv = pl->vertical_first ? fixed_h<true>(hc, vc) : fixed_h<false>(hc, vc);
-            const int FTHv = fv.th;
-            const int ntx = (ow + FTW - 1) / FTW, nty = (oh + FTHv - 1) / FTHv;
-            std::vector<int32_t> tix(ntx), tiy(nty);
-            int nix = 1, niy = 1;
-            for (int j = 0; j < ntx; ++j) {
-                int lo = 0x7fffffff, hi = -1;
-                for (int x = j * FTW; x < std::min(ow, (j + 1) * FTW); ++x) { lo = std::min(lo, pl->h.first[x]); hi = std::max(hi, pl->h.first[x] + hc - 1); }
-                tix[j] = lo; nix = std::max(nix, hi - lo + 1);
-            }
-            for (int j = 0; j < nty; ++j) {
-                int lo = 0x7fffffff, hi = -1;
-                for (int y = j * FTHv; y < std::min(oh, (j + 1) * FTHv); ++y) { lo = std::min(lo, pl->v.first[y]); hi = std::max(hi, pl->v.first[y] + vc - 1); }
-                tiy[j] = lo; niy = std::max(niy, hi - lo + 1);
-            }
-            const size_t fsmem = sizeof(float4) * ((size_t)nix * niy + (pl->vertical_first ? (size_t)FTHv * nix : (size_t)niy * FTW))
-                               + sizeof(int) * (FTW + FTHv) + sizeof(float) * ((size_t)FTW * (hc + 1) + (size_t)FTHv * (vc + 1));
-            if (fsmem <= 100 * 1024) {
-                // tile origins live behind the flag word in ctx->misc (re-uploaded per call: a few hundred bytes)
-                B2_CUDA(ctx, ctx->misc.reserve(4096 + sizeof(int32_t) * (size_t)(ntx + nty)));
-                int32_t *d_t = reinterpret_cast<int32_t *>(ctx->misc.as<char>() + 4096);
-                B2_CUDA(ctx, cudaMemcpyAsync(d_t, tix.data(), sizeof(int32_t) * ntx, cudaMemcpyHostToDevice, ctx->stream));
-                B2_CUDA(ctx, cudaMemcpyAsync(d_t + ntx, tiy.data(), sizeof(int32_t) * nty, cudaMemcpyHostToDevice, ctx->stream));
-                FixedGeom FG{nix, niy, d_t, d_t + ntx};
-                B2_CUDA(ctx, cudaFuncSetAttribute(fv.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-                const dim3 grid(ntx, nty, n_frames);
-                B2_KERNEL(ctx, "resample_fixed_kernel");
-                fv.fn<<<grid, fv.nt, fsmem, ctx->stream>>>(in, out, P, FG);
-                B2_LAUNCH_CHECK(ctx);
-                return B200TIMG_OK;
-            }
-        }
+        PlanarFn fn = planar_h<32, 3>(S.hc, S.vc);
+        B2_CUDA(ctx, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PLANAR_SMEM_CAP));
+        const dim3 grid(ntx, nty, n_frames);
+        B2_KERNEL(ctx, "resample_planar_kernel");
+        fn<<<grid, PNT, S.psmem, ctx->stream>>>(in, out, P, PG);
+        break;
+    }
+    case B200TIMG_SCALE_FIXED: {
+        const int ntx = (int)S.ftix.size(), nty = (int)S.ftiy.size();
+        // tile origins live behind the flag word in ctx->misc (re-uploaded per call: a few hundred bytes)
+        B2_CUDA(ctx, ctx->misc.reserve(4096 + sizeof(int32_t) * (size_t)(ntx + nty)));
+        int32_t *d_t = reinterpret_cast<int32_t *>(ctx->misc.as<char>() + 4096);
+        B2_CUDA(ctx, cudaMemcpyAsync(d_t, S.ftix.data(), sizeof(int32_t) * ntx, cudaMemcpyHostToDevice, ctx->stream));
+        B2_CUDA(ctx, cudaMemcpyAsync(d_t + ntx, S.ftiy.data(), sizeof(int32_t) * nty, cudaMemcpyHostToDevice, ctx->stream));
+        FixedGeom FG{S.fnix, S.fniy, d_t, d_t + ntx};
+        B2_CUDA(ctx, cudaFuncSetAttribute(S.fv.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FIXED_SMEM_CAP));
+        const dim3 grid(ntx, nty, n_frames);
+        B2_KERNEL(ctx, "resample_fixed_kernel");
+        S.fv.fn<<<grid, S.fv.nt, S.fsmem, ctx->stream>>>(in, out, P, FG);
+        break;
+    }
+    default: {
         // long filters: two 1-D passes over a float4 intermediate in global memory
         const size_t t_elems = pl->vertical_first ? (size_t)oh * iw : (size_t)ih * ow;
         const size_t o_tmp = 0, o_flag = (sizeof(float4) * t_elems * n_frames + 255) / 256 * 256;
@@ -1297,7 +1377,7 @@ int launch_scale(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int fmt
         B2_CUDA(ctx, cudaMemsetAsync(T.need_plain, 0, sizeof(int) * (size_t)n_frames, ctx->stream));
         const dim3 g2((ow + 31) / 32, (oh + 7) / 8, n_frames);
         for (int plain = 0; plain < 2; ++plain) {
-            if (pl->vertical_first) {
+            if (S.route == B200TIMG_SCALE_TP_V) {
                 const dim3 g1((iw + 255) / 256, oh, n_frames);
                 B2_KERNEL(ctx, plain ? "twopass_plain_kernels" : "twopass_v1_kernel");
                 if (plain) twopass_v1_kernel<true><<<g1, 256, 0, ctx->stream>>>(in, T); else twopass_v1_kernel<false><<<g1, 256, 0, ctx->stream>>>(in, T);
@@ -1307,37 +1387,23 @@ int launch_scale(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int fmt
                 B2_LAUNCH_CHECK(ctx);
             } else {
                 const dim3 g1((ow + 31) / 32, (ih + 7) / 8, n_frames);
-                // staged variant: window of a 32-column tile = first[tile start] .. max(first + count) over the tile
-                H1sGeom HG{1, pl->h.widest | 1};
-                for (int x0 = 0; x0 < ow; x0 += 32) {
-                    int hi = 0;
-                    for (int x = x0; x < std::min(ow, x0 + 32); ++x) hi = std::max(hi, pl->h.first[x] + pl->h.count[x]);
-                    HG.nwin = std::max(HG.nwin, hi - pl->h.first[x0]);
-                }
-                const size_t h1smem = sizeof(float4) * 8 * (size_t)HG.nwin + sizeof(float) * 32 * (size_t)HG.cpitch;
-                B2_KERNEL(ctx, plain ? "twopass_plain_kernels" : "twopass_h1_kernel");
-                // staging pays when the 32-column tiles are mostly full (4K -> 337 columns); with 67 columns the third
-                // tile stages a whole window for 3 outputs: plain kernel
-                const bool tiles_full = (long long)((ow + 31) / 32) * 32 * 100 <= (long long)ow * 115;
-                if (h1smem <= 72 * 1024 && tiles_full && !getenv("B200TIMG_NO_H1S")) {
+                if (S.route == B200TIMG_SCALE_TP_H1S) {
+                    B2_KERNEL(ctx, plain ? "twopass_plain_kernels" : "twopass_h1s_kernel");
                     if (plain) {
-                        B2_CUDA(ctx, cudaFuncSetAttribute(twopass_h1s_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 72 * 1024));
-                        twopass_h1s_kernel<true><<<g1, 256, h1smem, ctx->stream>>>(in, T, HG);
+                        B2_CUDA(ctx, cudaFuncSetAttribute(twopass_h1s_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)H1S_SMEM_CAP));
+                        twopass_h1s_kernel<true><<<g1, 256, S.h1smem, ctx->stream>>>(in, T, S.hg);
                     } else {
-                        B2_CUDA(ctx, cudaFuncSetAttribute(twopass_h1s_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 72 * 1024));
-                        twopass_h1s_kernel<false><<<g1, 256, h1smem, ctx->stream>>>(in, T, HG);
+                        B2_CUDA(ctx, cudaFuncSetAttribute(twopass_h1s_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)H1S_SMEM_CAP));
+                        twopass_h1s_kernel<false><<<g1, 256, S.h1smem, ctx->stream>>>(in, T, S.hg);
                     }
-                } else if (!tiles_full && ow <= 4096 && n_frames <= 65535 && !getenv("B200TIMG_NO_H1F")) {
-                    // few output columns: flat (row, column) mapping; rows per CTA chosen so that rows x ow fills whole 256-thread rounds
-                    int rows = 8; double best = 0.0;
-                    for (int r = 4; r <= 64; ++r) {
-                        const long long items = (long long)r * ow, slots = (items + 255) / 256 * 256;
-                        const double fill = (double)items / (double)slots;
-                        if (fill > best + 1e-9) { best = fill; rows = r; }
-                    }
-                    const dim3 gf((ih + rows - 1) / rows, n_frames);
-                    if (plain) twopass_h1f_kernel<true><<<gf, 256, 0, ctx->stream>>>(in, T, rows); else twopass_h1f_kernel<false><<<gf, 256, 0, ctx->stream>>>(in, T, rows);
-                } else if (plain) twopass_h1_kernel<true><<<g1, 256, 0, ctx->stream>>>(in, T); else twopass_h1_kernel<false><<<g1, 256, 0, ctx->stream>>>(in, T);
+                } else if (S.route == B200TIMG_SCALE_TP_H1F) {
+                    B2_KERNEL(ctx, plain ? "twopass_plain_kernels" : "twopass_h1f_kernel");
+                    const dim3 gf((ih + S.h1f_rows - 1) / S.h1f_rows, n_frames);
+                    if (plain) twopass_h1f_kernel<true><<<gf, 256, 0, ctx->stream>>>(in, T, S.h1f_rows); else twopass_h1f_kernel<false><<<gf, 256, 0, ctx->stream>>>(in, T, S.h1f_rows);
+                } else {
+                    B2_KERNEL(ctx, plain ? "twopass_plain_kernels" : "twopass_h1_kernel");
+                    if (plain) twopass_h1_kernel<true><<<g1, 256, 0, ctx->stream>>>(in, T); else twopass_h1_kernel<false><<<g1, 256, 0, ctx->stream>>>(in, T);
+                }
                 B2_LAUNCH_CHECK(ctx);
                 B2_KERNEL(ctx, plain ? "twopass_plain_kernels" : "twopass_2_kernel");
                 if (plain) twopass_2_kernel<false, true><<<g2, 256, 0, ctx->stream>>>(out, T); else twopass_2_kernel<false, false><<<g2, 256, 0, ctx->stream>>>(out, T);
@@ -1345,6 +1411,7 @@ int launch_scale(b200timg_ctx *ctx, const uint8_t *d_in, int iw, int ih, int fmt
             }
         }
         return B200TIMG_OK;
+    }
     }
     B2_LAUNCH_CHECK(ctx);
     return B200TIMG_OK;
@@ -1631,5 +1698,34 @@ extern "C" int b200timg_resample_plan(int in_w, int in_h, int out_w, int out_h, 
     if (count) memcpy(count, T.count.data(), sizeof(int32_t) * T.out_size);
     if (lead) memcpy(lead, T.lead.data(), sizeof(int32_t) * T.out_size);
     if (coeff) memcpy(coeff, T.coeff.data(), sizeof(float) * T.coeff.size());
+    return B200TIMG_OK;
+}
+
+// Host-only introspection of launch_scale's choice: the same scale_shape() call, every candidate evaluated.
+extern "C" int b200timg_scale_shape_of(int iw, int ih, int ow, int oh, int n_frames, int fast, int src_aligned16, int dst_aligned16,
+                                       b200timg_scale_shape *out) {
+    using namespace b200timg;
+    ResamplePlan pl;
+    if (!out || n_frames <= 0 || !build_resample_plan(iw, ih, ow, oh, &pl)) return B200TIMG_EINVAL;
+    if (!pl.copy_only && n_frames > 65535) return B200TIMG_EINVAL;                    // as launch_scale
+    const ScaleShape S = scale_shape(pl, iw, ih, ow, oh, n_frames, fast != 0, src_aligned16 != 0, dst_aligned16 != 0, true);
+    memset(out, 0, sizeof *out);
+    out->route = S.route; out->hc = S.hc; out->vc = S.vc; out->h_widest = pl.h.widest; out->v_widest = pl.v.widest;
+    out->vertical_first = pl.vertical_first; out->h_sequential = pl.h_sequential;
+    out->h_filter = (int)pl.h.filter; out->v_filter = (int)pl.v.filter; out->h_gather = pl.h.gather_mode; out->v_gather = pl.v.gather_mode;
+    out->h1f_rows = S.h1f_rows;
+    out->v3_tma = S.route == B200TIMG_SCALE_V3 && S.v3_tma;
+    out->planar_reuse = S.planar_reuse; out->v3_reuse = S.v3_reuse; out->tiles_full = S.tiles_full;
+    out->planar_smem = (int)S.psmem; out->v3_smem = (int)S.v3smem; out->fixed_smem = (int)S.fsmem; out->h1s_smem = (int)S.h1smem;
+    switch (S.route) {
+    case B200TIMG_SCALE_V3:
+        out->tiles_x = (int)S.tix3.size(); out->tiles_y = (int)S.tiy.size(); out->win_w = S.sp3; out->win_h = S.niy; break;
+    case B200TIMG_SCALE_PLANAR:
+        out->tiles_x = (int)S.tix.size(); out->tiles_y = (int)S.tiy.size(); out->win_w = S.nix; out->win_h = S.niy; break;
+    case B200TIMG_SCALE_FIXED:
+        out->tiles_x = (int)S.ftix.size(); out->tiles_y = (int)S.ftiy.size(); out->win_w = S.fnix; out->win_h = S.fniy; break;
+    case B200TIMG_SCALE_COPY4: case B200TIMG_SCALE_COPY: break;
+    default: out->tiles_x = (ow + 31) / 32; out->tiles_y = (oh + 7) / 8; break;
+    }
     return B200TIMG_OK;
 }
