@@ -253,9 +253,9 @@ int b200timg_sixel_batch(b200timg_ctx *ctx, const b200timg_batch *b, const uint8
  * src_offset that is not a multiple of 4, an odd out_w in quarter mode (the message names the frame), a YUV or
  * unknown src_fmt, B200TIMG_BILINEAR_SCALE, more than 2^31 - 1 row pairs or scaler work items in one call.
  * B200TIMG_FAST_SCALE is accepted and ignored: mixed batches always scale bit-exactly.
- * Out of scope: delta frames (a grid page has none, so there is no animation field), YUV sources, the bilinear
- * scaler, and the kitty / iTerm2 encoders (they build on b200timg_scale_mixed_dev's output).  The sixel encoder takes
- * mixed batches: b200timg_sixel_mixed_dev below. */
+ * Out of scope: delta frames (a grid page has none, so there is no animation field), YUV sources and the bilinear
+ * scaler.  The sixel encoder takes mixed batches (b200timg_sixel_mixed_dev below), and so do the kitty / iTerm2
+ * encoders (b200timg_graphics_mixed_dev, after b200timg_graphics further down). */
 typedef struct {
     uint64_t src_offset;        /* bytes from the batch's source pointer to this frame's first pixel; multiple of 4 */
     int src_w, src_h;           /* source geometry of this image */
@@ -498,6 +498,27 @@ size_t b200timg_graphics_size(const b200timg_graphics *g, int w, int h, uint32_t
 int b200timg_graphics_batch_dev(b200timg_ctx *ctx, const b200timg_batch *b, const b200timg_graphics *g,
                                 const uint8_t *d_src, char *d_out, size_t out_cap, uint64_t *d_offsets);
 int b200timg_graphics_batch(b200timg_ctx *ctx, const b200timg_batch *b, const b200timg_graphics *g,
+                            const uint8_t *src, char *out, size_t out_cap, uint64_t *offsets);
+/* Mixed batches (a `-pk` / `-pi` grid page, b200timg_mixed_batch above): scale -> compose -> PNG -> framing of every
+ * frame in one call.  Frame f's bytes are exactly those of b200timg_graphics_batch_dev on a one-frame b200timg_batch of
+ * that image with the page's compose options, flags = 0, the same protocol, rgb24 and cell size, id ids[f] and, for
+ * B200TIMG_KITTY_TMUX, indent_cells = frames[f].x_indent_cells -- whatever the frame's place in the batch, the batch size
+ * or the variant called, for all three protocols with and without B200TIMG_DEFLATE.
+ * Per frame: x_indent_cells is the tmux placeholder grid's indent (x / cell_x_px of that image's
+ * KittyGraphicsCanvas::Send: column offset plus centering); g->indent_cells is not read.  Shared by the page: g->ids
+ * holds n_frames ids (either kitty form), rgb24, the cell size and the compose options apply to every frame.  The block
+ * flags are ignored; B200TIMG_FAST_SCALE is accepted and ignored.
+ * Rejected with B200TIMG_EINVAL: everything the mixed batches above reject, what b200timg_graphics_batch rejects
+ * about the protocol description (unknown protocol or 3 | B200TIMG_DEFLATE, ids == NULL for kitty, a non-positive cell
+ * size for tmux) and a frame whose PNG does not fit one IDAT chunk (the message names the frame).
+ * A call runs a fixed number of kernels whatever the page's geometries; tables, descriptors, ids and (stored blocks)
+ * offsets go up in one copy.  The _dev variant follows the OUTPUT CAPACITY CONTRACT: stored blocks, d_offsets is the
+ * running sum of b200timg_graphics_size per frame (computed on the host); B200TIMG_DEFLATE, it comes from the device
+ * as in the uniform batch.  The host variant returns B200TIMG_ENOSPC with offsets[] complete and nothing written at or
+ * beyond out_cap: with stored blocks before launching anything, with B200TIMG_DEFLATE after reading the offsets back. */
+int b200timg_graphics_mixed_dev(b200timg_ctx *ctx, const b200timg_mixed_batch *b, const b200timg_graphics *g,
+                                const uint8_t *d_src, char *d_out, size_t out_cap, uint64_t *d_offsets);
+int b200timg_graphics_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *b, const b200timg_graphics *g,
                             const uint8_t *src, char *out, size_t out_cap, uint64_t *offsets);
 
 /* ======================= K7: gather of the encoded frames over NCCL ==============================

@@ -140,6 +140,10 @@ ABI = {
                                               C.c_size_t, C.c_void_p]),
     "b200timg_graphics_batch": (C.c_int, [C.c_void_p, C.POINTER(Batch), C.POINTER(Graphics), C.c_void_p, C.c_void_p,
                                           C.c_size_t, C.c_void_p]),
+    "b200timg_graphics_mixed_dev": (C.c_int, [C.c_void_p, C.POINTER(MixedBatch), C.POINTER(Graphics), C.c_void_p, C.c_void_p,
+                                              C.c_size_t, C.c_void_p]),
+    "b200timg_graphics_mixed": (C.c_int, [C.c_void_p, C.POINTER(MixedBatch), C.POINTER(Graphics), C.c_void_p, C.c_void_p,
+                                          C.c_size_t, C.c_void_p]),
     "b200timg_gather_unique_id": (C.c_int, [C.c_char_p]),
     "b200timg_gather_init": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int, C.c_int]),
     "b200timg_gather_attach": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
@@ -589,4 +593,49 @@ class Context:
             d_offsets = torch.empty(n + 1, dtype=torch.int64, device=d_src.device)
         self._chk(lib().b200timg_graphics_batch_dev(self.h, C.byref(b), C.byref(g), d_src.data_ptr(), d_out.data_ptr(),
                                                     out_cap, d_offsets.data_ptr()))
+        return d_out, d_offsets
+
+    @staticmethod
+    def graphics_mixed_bound(b, g):
+        """Bytes of a kitty / iTerm2 mixed batch with stored blocks (the exact size; an upper bound with DEFLATE): the sum
+        of b200timg_graphics_size over the frames, each with its own indent and id."""
+        kitty = (g.protocol & ~DEFLATE) != ITERM2
+        total = 0
+        for f in range(b.n_frames):
+            F = b.frames[f]
+            gf = Graphics(g.protocol, g.rgb24, None, g.cell_x_px, g.cell_y_px, F.x_indent_cells)
+            total += lib().b200timg_graphics_size(C.byref(gf), F.out_w, F.out_h, int(g.ids[f]) if kitty else 0)
+        return total
+
+    def graphics_mixed(self, images, outs, protocol, rgb24=False, ids=None, indents=None, cell=None, deflate=False,
+                       with_offsets=False, **compose):
+        """b200timg_graphics_mixed (host buffers): each frame's framed kitty / iTerm2 text, as a list of bytes (and the
+        offsets with with_offsets).  ids: one kitty image id per frame; indents: each frame's tmux placeholder indent
+        (x_indent_cells); cell: (cell_x_px, cell_y_px) of the tmux form; compose: has_bg, bg, pattern, ... as mixed_batch."""
+        flat, offs = pack_mixed(images)
+        b, keep = mixed_batch([im.shape for im in images], outs, offs, indents, compose.pop("flags", 0), **compose)
+        g, keep_ids = graphics(protocol | (DEFLATE if deflate else 0), rgb24, ids, cell)
+        n = len(outs)
+        cap = max(1, self.graphics_mixed_bound(b, g))
+        out = np.empty(cap, np.uint8)
+        o = np.zeros(n + 1, np.uint64)
+        self._chk(lib().b200timg_graphics_mixed(self.h, C.byref(b), C.byref(g), flat.ctypes.data, out.ctypes.data, cap,
+                                                o.ctypes.data))
+        res = [out[int(o[i]):int(o[i + 1])].tobytes() for i in range(n)]
+        return (res, o) if with_offsets else res
+
+    def graphics_mixed_dev(self, d_src, b, g, d_out=None, out_cap=None, d_offsets=None):
+        """b200timg_graphics_mixed_dev on a packed source tensor (see pack_mixed / mixed_batch) with a protocol description
+        from graphics() (keep its id array alive): returns (d_out, d_offsets) after the (asynchronous) call --
+        device_sync() before reading them; d_out defaults to graphics_mixed_bound."""
+        import torch
+        n = b.n_frames
+        if d_out is None:
+            d_out = torch.empty(max(1, self.graphics_mixed_bound(b, g)), dtype=torch.uint8, device=d_src.device)
+        if out_cap is None:
+            out_cap = d_out.numel()
+        if d_offsets is None:
+            d_offsets = torch.empty(n + 1, dtype=torch.int64, device=d_src.device)
+        self._chk(lib().b200timg_graphics_mixed_dev(self.h, C.byref(b), C.byref(g), d_src.data_ptr(), d_out.data_ptr(), out_cap,
+                                                    d_offsets.data_ptr()))
         return d_out, d_offsets

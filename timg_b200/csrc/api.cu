@@ -510,15 +510,21 @@ int b200timg_sixel_batch_dev(b200timg_ctx *ctx, const b200timg_batch *b, const u
 }
 
 // ---- kitty / iTerm2 batches ------------------------------------------------------------------
-static int validate_graphics(b200timg_ctx *ctx, const b200timg_batch *b, const b200timg_graphics *g) {
+// the protocol description; mixed batches take the tmux indent per frame, so g->indent_cells is read for uniform ones only
+static int validate_protocol(b200timg_ctx *ctx, const b200timg_graphics *g, bool uses_indent) {
     if (!g) return ctx->fail(B200TIMG_EINVAL, "graphics: null protocol description");
     const int protocol = g->protocol & ~B200TIMG_DEFLATE;
     if (protocol != B200TIMG_KITTY && protocol != B200TIMG_ITERM2 && protocol != B200TIMG_KITTY_TMUX)
         return ctx->fail(B200TIMG_EINVAL, "graphics: unknown protocol %d", g->protocol);
     if (protocol != B200TIMG_ITERM2 && !g->ids) return ctx->fail(B200TIMG_EINVAL, "graphics: kitty needs one image id per frame (ids is NULL)");
-    if (protocol == B200TIMG_KITTY_TMUX && (g->cell_x_px <= 0 || g->cell_y_px <= 0 || g->indent_cells < 0))
+    if (protocol == B200TIMG_KITTY_TMUX && (g->cell_x_px <= 0 || g->cell_y_px <= 0 || (uses_indent && g->indent_cells < 0)))
         return ctx->fail(B200TIMG_EINVAL, "graphics: tmux placeholders need a positive cell size and indent >= 0 (cell %dx%d, indent %d)",
-                         g->cell_x_px, g->cell_y_px, g->indent_cells);
+                         g->cell_x_px, g->cell_y_px, uses_indent ? g->indent_cells : 0);
+    return B200TIMG_OK;
+}
+
+static int validate_graphics(b200timg_ctx *ctx, const b200timg_batch *b, const b200timg_graphics *g) {
+    B2_TRY(validate_protocol(ctx, g, true));
     if (b->animation != 0) return ctx->fail(B200TIMG_EINVAL, "graphics: kitty / iTerm2 frames have no delta encoding (animation must be 0)");
     if (b200timg_png_size(b->out_w, b->out_h, g->rgb24) > 0x7fffffffu)
         return ctx->fail(B200TIMG_EINVAL, "graphics: the PNG of a %dx%d frame does not fit one IDAT chunk", b->out_w, b->out_h);
@@ -870,6 +876,81 @@ int b200timg_sixel_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *b, const
     const size_t total = (size_t)offsets[n];
     if (total > bound) return ctx->fail(B200TIMG_ECUDA, "sixel mixed batch: encoded size %zu exceeds the bound %zu", total, bound);
     if (total > out_cap) return ctx->fail(B200TIMG_ENOSPC, "sixel mixed batch: need %zu bytes (have %zu)", total, out_cap);
+    if (total) B2_TRY(download(ctx, out, ctx->out_stage.p, total));
+    return sync(ctx);
+}
+
+// Only the fields a mixed page reads, so that nothing else of the caller's description reaches the kernels.
+static b200timg_graphics graphics_mixed_desc(const b200timg_graphics *g) {
+    b200timg_graphics r = {};
+    r.protocol = g->protocol;
+    r.rgb24 = g->rgb24;
+    r.ids = (g->protocol & ~B200TIMG_DEFLATE) != B200TIMG_ITERM2 ? g->ids : nullptr;
+    if ((g->protocol & ~B200TIMG_DEFLATE) == B200TIMG_KITTY_TMUX) { r.cell_x_px = g->cell_x_px; r.cell_y_px = g->cell_y_px; }
+    return r;
+}
+
+int b200timg_graphics_mixed_dev(b200timg_ctx *ctx, const b200timg_mixed_batch *b, const b200timg_graphics *g,
+                                const uint8_t *d_src, char *d_out, size_t out_cap, uint64_t *d_offsets) {
+    B2_TRY(check_ctx(ctx));
+    B2_TRY(validate_mixed(ctx, b, false));
+    B2_TRY(validate_protocol(ctx, g, false));
+    if (!d_src || !d_out || !d_offsets) return ctx->fail(B200TIMG_EINVAL, "mixed batch: null pointer");
+    if (reinterpret_cast<uintptr_t>(d_src) & 3) return ctx->fail(B200TIMG_EINVAL, "mixed batch: pixel buffers must be 4-byte aligned");
+    const b200timg_graphics gr = graphics_mixed_desc(g);
+    MixedPlan mp;
+    B2_TRY(plan_scale_mixed(ctx, b, mp));
+    B2_TRY(plan_graphics_mixed(ctx, b, gr, mp));
+    ctx->resident_fb = nullptr;
+    B2_CUDA(ctx, ctx->fb_scaled.reserve((size_t)mp.out_px * 4));
+    B2_TRY(mixed_upload(ctx, mp));
+    const ComposeSpec cs = make_compose_spec(b->has_bg, b->bg, b->pattern, b->pattern_w, b->pattern_h);
+    uint8_t *d_fb = ctx->fb_scaled.as<uint8_t>();
+    const char *d_arena = ctx->mixed_arena.as<char>();
+    B2_TRY(launch_scale_mixed(ctx, mp, d_arena, d_src, d_fb, b->n_frames, b->src_fmt == B200TIMG_FMT_RGB32, cs));
+    return launch_graphics_mixed(ctx, mp, d_arena, d_fb, b->n_frames, gr, d_offsets, d_out, out_cap);
+}
+
+// Host buffers.  Stored blocks: every size is known before the call, so ENOSPC comes before anything runs.
+// B200TIMG_DEFLATE: staging bounded by the stored sizes, offsets read back, then exactly the encoded bytes (or nothing,
+// with ENOSPC and the offsets complete).
+int b200timg_graphics_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *b, const b200timg_graphics *g,
+                            const uint8_t *src, char *out, size_t out_cap, uint64_t *offsets) {
+    B2_TRY(check_ctx(ctx));
+    B2_TRY(validate_mixed(ctx, b, false));
+    B2_TRY(validate_protocol(ctx, g, false));
+    if (!src || !out || !offsets) return ctx->fail(B200TIMG_EINVAL, "mixed batch: null pointer");
+    const int n = b->n_frames;
+    const bool deflate = (g->protocol & B200TIMG_DEFLATE) != 0, kitty = (g->protocol & ~B200TIMG_DEFLATE) != B200TIMG_ITERM2;
+    size_t src_bytes = 0, bound = 0;
+    std::vector<uint64_t> sized(n + 1, 0);
+    for (int f = 0; f < n; ++f) {
+        const b200timg_frame &F = b->frames[f];
+        src_bytes = std::max(src_bytes, (size_t)F.src_offset + (size_t)F.src_w * F.src_h * 4);
+        b200timg_graphics gf = graphics_mixed_desc(g);
+        gf.indent_cells = F.x_indent_cells;
+        if (b200timg_png_size(F.out_w, F.out_h, g->rgb24) > 0x7fffffffu)
+            return ctx->fail(B200TIMG_EINVAL, "graphics mixed batch: frame %d: the PNG of a %dx%d frame does not fit one IDAT chunk", f,
+                             F.out_w, F.out_h);
+        sized[f + 1] = sized[f] + b200timg_graphics_size(&gf, F.out_w, F.out_h, kitty ? g->ids[f] : 0);
+    }
+    bound = (size_t)sized[n];
+    if (!deflate) {
+        memcpy(offsets, sized.data(), sizeof(uint64_t) * (n + 1));
+        if (bound > out_cap) return ctx->fail(B200TIMG_ENOSPC, "graphics mixed batch: need %zu bytes (have %zu)", bound, out_cap);
+    }
+    B2_CUDA(ctx, ctx->in_stage.reserve(src_bytes));
+    B2_CUDA(ctx, ctx->out_stage.reserve(std::max<size_t>(bound, 1)));
+    B2_CUDA(ctx, ctx->offsets.reserve((size_t)(n + 1) * sizeof(uint64_t)));
+    B2_CUDA(ctx, ctx->pinned.reserve((size_t)(n + 1) * sizeof(uint64_t)));
+    B2_TRY(upload(ctx, ctx->in_stage.p, src, src_bytes));
+    B2_TRY(b200timg_graphics_mixed_dev(ctx, b, g, ctx->in_stage.as<uint8_t>(), ctx->out_stage.as<char>(), bound, ctx->offsets.as<uint64_t>()));
+    B2_TRY(download(ctx, ctx->pinned.p, ctx->offsets.p, (size_t)(n + 1) * sizeof(uint64_t)));
+    B2_TRY(sync(ctx));
+    memcpy(offsets, ctx->pinned.p, (size_t)(n + 1) * sizeof(uint64_t));
+    const size_t total = (size_t)offsets[n];
+    if (total > bound) return ctx->fail(B200TIMG_ECUDA, "graphics mixed batch: encoded size %zu exceeds the bound %zu", total, bound);
+    if (total > out_cap) return ctx->fail(B200TIMG_ENOSPC, "graphics mixed batch: need %zu bytes (have %zu)", total, out_cap);
     if (total) B2_TRY(download(ctx, out, ctx->out_stage.p, total));
     return sync(ctx);
 }

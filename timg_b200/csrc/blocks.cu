@@ -181,16 +181,6 @@ struct BlocksParams {
 
 constexpr int BT = 256;
 
-// The frame that owns flat item `item`: the last f with start[f] <= item (frames without items share their start).
-__device__ __forceinline__ int mixed_owner(const unsigned *__restrict__ start, int n, unsigned item) {
-    int lo = 0, hi = n - 1;
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (start[mid] <= item) lo = mid; else hi = mid - 1;
-    }
-    return lo;
-}
-
 // Where a CTA's row pair and its frame live.  The pass bodies below read every per-frame quantity through one of
 // these accessors:
 //   UniformGeom  a b200timg_batch: every frame has P's geometry, frame f at fb + f * P.frame_px, records frame-major

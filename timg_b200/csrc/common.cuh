@@ -298,6 +298,51 @@ struct MixedPlan {
     unsigned sixel_bands = 0, sixel_ctas = 0;      // flat (frame, band) and (frame, dither CTA) items
     int sixel_nwarps = 0, sixel_wmax = 0, sixel_split = 0;
     size_t sixel_pal_smem = 0, sixel_ent = 0, sixel_idx = 0, sixel_bnd = 0, sixel_scr = 0, sixel_prog = 0;
+    // kitty / iTerm2 encoder (plan_graphics_mixed): arena offsets of its descriptors, item starts, ids and offsets, the
+    // lengths of its flat item lists and the sizes of its scratch
+    size_t o_gfx = 0, o_gchk = 0, o_gtile = 0, o_ggrid = 0, o_gseg = 0, o_graw = 0, o_gpiece = 0, o_gids = 0, o_goffs = 0;
+    unsigned gfx_chk = 0, gfx_tiles = 0, gfx_grid = 0, gfx_segs = 0, gfx_pieces = 0;
+    unsigned long long gfx_raw = 0, gfx_raw_slots = 0, gfx_png_slots = 0;
+    std::vector<uint64_t> gfx_offsets;             // stored blocks: [n+1] running sum of the frame sizes
+};
+
+// The frame that owns flat item `item` of a mixed call's list: the last f with start[f] <= item (frames without items
+// share their start).
+template <class T>
+__device__ __forceinline__ int mixed_owner(const T *__restrict__ start, int n, T item) {
+    int lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (start[mid] <= item) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
+// ---- kitty / iTerm2 (png.cu, deflate.cu) -----------------------------------------------------------------------
+struct PngGeom {
+    int w, h, bpp;                 // bpp 4 (RGBA, colour type 6) or 3 (RGB, colour type 2)
+    long long row_bytes;           // 1 + w*bpp
+    long long raw_len;             // h * row_bytes : the filtered scanline stream
+    long long nblocks;             // stored deflate blocks of <= 65535 bytes
+    long long zlib_len;            // 2 + 5*nblocks + raw_len + 4
+    long long png_len;             // 8 + 25 + 12 + zlib_len + 12
+    long long idat_data_off;       // offset of the first zlib byte inside the PNG
+};
+struct GfxSpec {
+    int protocol;                           // B200TIMG_KITTY, B200TIMG_ITERM2 or B200TIMG_KITTY_TMUX
+    int w, h;
+    long long png_len, tiles;
+    int cols, rows, indent;                 // tmux form: the placeholder grid (kitty-canvas.cc:174-176), else 0
+};
+// One frame of a mixed kitty / iTerm2 batch (plan_graphics_mixed, png.cu).  The tile count and the placeholder grid's
+// cols, rows and indent are in s; with B200TIMG_DEFLATE, s describes the stored-size bound.
+struct __align__(16) MixedGfxFrame {
+    PngGeom g;
+    GfxSpec s;
+    unsigned long long fb;         // first byte of the scaled frame in launch_scale_mixed's output
+    long long raw_off, png_off;    // B200TIMG_DEFLATE: the frame's scanline slot in ctx->dfl_raw, PNG slot in ctx->dfl_png
+    unsigned seg0;                 // B200TIMG_DEFLATE: its first 65535-byte segment in the call's flat segment list
+    uint32_t ihdr;                 // CRC-32 of its IHDR chunk
 };
 // appends bytes at a 16-byte boundary of the arena and returns their offset
 inline size_t mixed_put(std::vector<char> &a, const void *p, size_t bytes) {
@@ -322,5 +367,16 @@ int launch_pad_mixed(b200timg_ctx *ctx, const MixedPlan &mp, const char *d_arena
 int plan_sixel_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *b, MixedPlan &mp);
 int launch_sixel_mixed(b200timg_ctx *ctx, const MixedPlan &mp, const char *d_arena, const uint8_t *d_fb, int n_frames,
                        char *d_out, size_t out_cap, uint64_t *d_offsets);
+// kitty / iTerm2 text of the composed frames of a plan made without sixel_rows; plan_graphics_mixed adds the encoder's
+// descriptors, item lists, ids and (stored blocks) offsets to the arena
+int plan_graphics_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *b, const b200timg_graphics &gr, MixedPlan &mp);
+int launch_graphics_mixed(b200timg_ctx *ctx, const MixedPlan &mp, const char *d_arena, const uint8_t *d_fb, int n_frames,
+                          const b200timg_graphics &gr, uint64_t *d_offsets, char *d_out, size_t out_cap);
+// deflate.cu over the flat segment list of a mixed batch (seg_start[n_frames + 1], frames' slots in desc)
+int launch_deflate_mixed(b200timg_ctx *ctx, const uint8_t *d_raw, const MixedGfxFrame *d_desc, const unsigned *d_seg_start,
+                         int n_frames, unsigned n_segs, uint8_t *d_scratch, DeflateSeg *d_info);
+int launch_deflate_pack_mixed(b200timg_ctx *ctx, const uint8_t *d_raw, const MixedGfxFrame *d_desc, const unsigned *d_seg_start,
+                              int n_frames, unsigned n_segs, const uint8_t *d_scratch, const DeflateSeg *d_info,
+                              const unsigned long long *d_start, uint8_t *d_png, int zoff);
 
 }  // namespace b200timg

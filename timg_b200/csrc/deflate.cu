@@ -151,18 +151,43 @@ __device__ void huff_codes(const uint8_t *len, int n, uint16_t *code) {
         if (len[i]) code[i] = (uint16_t)(__brev(next[len[i]]++) >> (32 - len[i]));
 }
 
-__global__ void __launch_bounds__(32 * DFL_WARPS)
-deflate_segment_kernel(const uint8_t *__restrict__ raw, long long raw_stride, int raw_len, int n_frames, int nseg,
-                       uint32_t *__restrict__ tokens, uint8_t *__restrict__ scratch, DeflateSeg *__restrict__ info) {
+// Where segment t of the flat segment list lives: its frame's scanline stream R (raw_len bytes), its index k in that
+// frame, the frame's segment count and PNG slot.
+//   DflUniform  a b200timg_batch: nseg segments per frame, frame f's stream at raw + f * raw_stride, PNG at f * png_stride
+//   DflMixed    a mixed batch: frame f's segments seg_start[f] .. seg_start[f + 1] - 1, its slots in desc[f]
+struct DflItem { const uint8_t *R; int raw_len, k, nseg; long long png0; };
+struct DflUniform {
+    const uint8_t *raw; long long raw_stride; int raw_len, n_frames, nseg; long long png_stride;
+    __device__ __forceinline__ long long total() const { return (long long)n_frames * nseg; }
+    __device__ __forceinline__ DflItem at(long long t) const {
+        const int f = (int)(t / nseg), k = (int)(t - (long long)f * nseg);
+        return DflItem{raw + f * raw_stride, raw_len, k, nseg, f * png_stride};
+    }
+};
+struct DflMixed {
+    const uint8_t *raw; const MixedGfxFrame *desc; const unsigned *seg_start; int n_frames;
+    __device__ __forceinline__ long long total() const { return seg_start[n_frames]; }
+    __device__ __forceinline__ DflItem at(long long t) const {
+        const int f = mixed_owner(seg_start, n_frames, (unsigned)t);
+        const MixedGfxFrame &D = desc[f];
+        return DflItem{raw + D.raw_off, (int)D.g.raw_len, (int)(t - seg_start[f]), (int)D.g.nblocks, D.png_off};
+    }
+};
+
+template <class A>
+__device__ __forceinline__ void deflate_segment_body(const A &a, uint32_t *__restrict__ tokens, uint8_t *__restrict__ scratch,
+                                                     DeflateSeg *__restrict__ info) {
     extern __shared__ __align__(16) uint8_t dfl_smem[];
     const unsigned FULL = 0xffffffffu;
     const int lane = threadIdx.x & 31;
     DflWarp &w = reinterpret_cast<DflWarp *>(dfl_smem)[threadIdx.x >> 5];
     const long long gw = (long long)blockIdx.x * DFL_WARPS + (threadIdx.x >> 5), nw = (long long)gridDim.x * DFL_WARPS;
     uint32_t *tok = tokens + gw * DFL_SEG;
-    for (long long t = gw; t < (long long)n_frames * nseg; t += nw) {
-        const int f = (int)(t / nseg), k = (int)(t - (long long)f * nseg);
-        const uint8_t *R = raw + f * raw_stride;
+    const long long total = a.total();
+    for (long long t = gw; t < total; t += nw) {
+        const DflItem it = a.at(t);
+        const uint8_t *R = it.R;
+        const int raw_len = it.raw_len, k = it.k;
         const int s0 = k * DFL_SEG, n = min(DFL_SEG, raw_len - s0), end = s0 + n;
         for (int i = lane; i < (1 << DFL_HBITS); i += 32) w.head[i] = 0;
         for (int i = lane; i < DFL_NSYM; i += 32) w.freq[i] = 0;
@@ -302,23 +327,33 @@ deflate_segment_kernel(const uint8_t *__restrict__ raw, long long raw_stride, in
         __syncwarp();
     }
 }
+__global__ void __launch_bounds__(32 * DFL_WARPS)
+deflate_segment_kernel(const uint8_t *__restrict__ raw, long long raw_stride, int raw_len, int n_frames, int nseg,
+                       uint32_t *__restrict__ tokens, uint8_t *__restrict__ scratch, DeflateSeg *__restrict__ info) {
+    deflate_segment_body(DflUniform{raw, raw_stride, raw_len, n_frames, nseg, 0}, tokens, scratch, info);
+}
+__global__ void __launch_bounds__(32 * DFL_WARPS)
+deflate_segment_mixed_kernel(const uint8_t *__restrict__ raw, const MixedGfxFrame *__restrict__ desc, const unsigned *__restrict__ seg_start,
+                             int n_frames, uint32_t *__restrict__ tokens, uint8_t *__restrict__ scratch, DeflateSeg *__restrict__ info) {
+    deflate_segment_body(DflMixed{raw, desc, seg_start, n_frames}, tokens, scratch, info);
+}
 
 // One CTA per segment (grid-stride): the segment's block at bit 8 * zoff + start[t] of its frame's PNG slot (slot
 // zeroed beforehand).  Words the block covers entirely are stored, the two it shares with its neighbours are OR'ed.
-__global__ void __launch_bounds__(256)
-deflate_pack_kernel(const uint8_t *__restrict__ raw, long long raw_stride, int raw_len, int n_frames, int nseg,
-                    const uint8_t *__restrict__ scratch, const DeflateSeg *__restrict__ info,
-                    const unsigned long long *__restrict__ start, uint8_t *__restrict__ png, long long png_stride, int zoff) {
-    for (long long t = blockIdx.x; t < (long long)n_frames * nseg; t += gridDim.x) {
-        const int f = (int)(t / nseg), k = (int)(t - (long long)f * nseg);
+template <class A_>
+__device__ __forceinline__ void deflate_pack_body(const A_ &a, const uint8_t *__restrict__ scratch, const DeflateSeg *__restrict__ info,
+                                                  const unsigned long long *__restrict__ start, uint8_t *__restrict__ png, int zoff) {
+    for (long long t = blockIdx.x; t < a.total(); t += gridDim.x) {
+        const DflItem it = a.at(t);
+        const int raw_len = it.raw_len, k = it.k, nseg = it.nseg;
         const DeflateSeg sg = info[t];
         const uint32_t n = (uint32_t)min(DFL_SEG, raw_len - k * DFL_SEG);
         const unsigned long long A = 8ull * zoff + start[t];
         const unsigned long long P = (A + 10) & ~7ull;               // a stored block's LEN, after 3 bits and padding
         const unsigned long long B = sg.stored ? P + 32 + 8ull * n : A + sg.bits;
-        uint32_t *D = reinterpret_cast<uint32_t *>(png + f * png_stride);
+        uint32_t *D = reinterpret_cast<uint32_t *>(png + it.png0);
         const uint32_t *S = reinterpret_cast<const uint32_t *>(scratch + t * DFL_SLOT);
-        const uint8_t *Rs = raw + f * raw_stride + (long long)k * DFL_SEG;
+        const uint8_t *Rs = it.R + (long long)k * DFL_SEG;
         for (unsigned long long wd = (A >> 5) + threadIdx.x; wd <= (B - 1) >> 5; wd += blockDim.x) {
             const unsigned long long lo = wd * 32;
             uint32_t v = 0;
@@ -345,6 +380,18 @@ deflate_pack_kernel(const uint8_t *__restrict__ raw, long long raw_stride, int r
         }
     }
 }
+__global__ void __launch_bounds__(256)
+deflate_pack_kernel(const uint8_t *__restrict__ raw, long long raw_stride, int raw_len, int n_frames, int nseg,
+                    const uint8_t *__restrict__ scratch, const DeflateSeg *__restrict__ info,
+                    const unsigned long long *__restrict__ start, uint8_t *__restrict__ png, long long png_stride, int zoff) {
+    deflate_pack_body(DflUniform{raw, raw_stride, raw_len, n_frames, nseg, png_stride}, scratch, info, start, png, zoff);
+}
+__global__ void __launch_bounds__(256)
+deflate_pack_mixed_kernel(const uint8_t *__restrict__ raw, const MixedGfxFrame *__restrict__ desc, const unsigned *__restrict__ seg_start,
+                          int n_frames, const uint8_t *__restrict__ scratch, const DeflateSeg *__restrict__ info,
+                          const unsigned long long *__restrict__ start, uint8_t *__restrict__ png, int zoff) {
+    deflate_pack_body(DflMixed{raw, desc, seg_start, n_frames}, scratch, info, start, png, zoff);
+}
 
 int launch_deflate(b200timg_ctx *ctx, const uint8_t *d_raw, long long raw_stride, int raw_len, int n_frames, int nseg,
                    uint8_t *d_scratch, DeflateSeg *d_info) {
@@ -366,6 +413,29 @@ int launch_deflate_pack(b200timg_ctx *ctx, const uint8_t *d_raw, long long raw_s
     B2_KERNEL(ctx, "deflate_pack_kernel");
     deflate_pack_kernel<<<(unsigned)std::min<long long>(items, (long long)ctx->sm_count * 16), 256, 0, ctx->stream>>>(
         d_raw, raw_stride, raw_len, n_frames, nseg, d_scratch, d_info, d_start, d_png, png_stride, zoff);
+    B2_LAUNCH_CHECK(ctx);
+    return B200TIMG_OK;
+}
+
+// The same two passes over a mixed batch's flat segment list: the launch shapes follow the list's length as above.
+int launch_deflate_mixed(b200timg_ctx *ctx, const uint8_t *d_raw, const MixedGfxFrame *d_desc, const unsigned *d_seg_start,
+                         int n_frames, unsigned n_segs, uint8_t *d_scratch, DeflateSeg *d_info) {
+    const long long ctas = std::min<long long>((n_segs + DFL_WARPS - 1) / DFL_WARPS, (long long)ctx->sm_count * 2);
+    B2_CUDA(ctx, ctx->dfl_tokens.reserve((size_t)ctas * DFL_WARPS * DFL_SEG * sizeof(uint32_t)));
+    B2_CUDA(ctx, cudaFuncSetAttribute(deflate_segment_mixed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DFL_SMEM));
+    B2_KERNEL(ctx, "deflate_segment_mixed_kernel");
+    deflate_segment_mixed_kernel<<<(unsigned)ctas, 32 * DFL_WARPS, DFL_SMEM, ctx->stream>>>(d_raw, d_desc, d_seg_start, n_frames,
+                                                                                          ctx->dfl_tokens.as<uint32_t>(), d_scratch, d_info);
+    B2_LAUNCH_CHECK(ctx);
+    return B200TIMG_OK;
+}
+
+int launch_deflate_pack_mixed(b200timg_ctx *ctx, const uint8_t *d_raw, const MixedGfxFrame *d_desc, const unsigned *d_seg_start,
+                              int n_frames, unsigned n_segs, const uint8_t *d_scratch, const DeflateSeg *d_info,
+                              const unsigned long long *d_start, uint8_t *d_png, int zoff) {
+    B2_KERNEL(ctx, "deflate_pack_mixed_kernel");
+    deflate_pack_mixed_kernel<<<(unsigned)std::min<long long>(n_segs, (long long)ctx->sm_count * 16), 256, 0, ctx->stream>>>(
+        d_raw, d_desc, d_seg_start, n_frames, d_scratch, d_info, d_start, d_png, zoff);
     B2_LAUNCH_CHECK(ctx);
     return B200TIMG_OK;
 }

@@ -1,6 +1,7 @@
 #!/usr/bin/env python
-"""Mixed batches on the GPU: a `timg --grid` page of differently sized images, block- or sixel-encoded in one call
-(b200timg_blocks_mixed_dev, b200timg_sixel_mixed_dev) against the ways to send it without one.  One JSON line per page.
+"""Mixed batches on the GPU: a `timg --grid` page of differently sized images, block-, sixel- or kitty-encoded in one call
+(b200timg_blocks_mixed_dev, b200timg_sixel_mixed_dev, b200timg_graphics_mixed_dev) against the ways to send it without
+one.  One JSON line per page.
 
   python tools/bench_mixed.py [--steps K] [--warmup W] [--only NAME]
 
@@ -8,16 +9,22 @@
   grid4x4-half     --grid=4x4 -g300x100 -p half: 16 images fitted to 75 x 50 px (larger outputs per image)
   grid4x4-sixel    --grid=4x4 -g300x100 -p sixel at 9 x 18 px cells: 16 images fitted to 675 x 450 px
   grid8x8-sixel    --grid=8x8 -g300x100 -p sixel at 9 x 18 px cells: 64 images fitted to 337 x 225 px
+  grid8x8-kitty[-deflate]  --grid=8x8 -g300x100 -p kitty at 9 x 18 px cells (tmux off, rgb24): 64 images fitted to
+                   337 x 225 px, stored-block PNGs (timg's --compress 0) or B200TIMG_DEFLATE (its default, level 1)
+  grid4x4-kitty[-deflate]  the same at --grid=4x4: 16 images fitted to 675 x 450 px
 Source sizes cycle through 3840x2160, 2160x3840, 4032x3024, 3000x2000, 1920x1080, 1280x720, 1080x1080 and 640x480
 (every image's pixels distinct); indents are the renderer's column offsets (src/renderer.cc:124-142).
 
 Timed, alternating within each step, every call ending in a device-wide synchronise:
-  (a) mixed     one b200timg_blocks_mixed_dev (sixel pages: b200timg_sixel_mixed_dev) call for the page
-  (b) per_image one b200timg_blocks_batch_dev (b200timg_sixel_batch_dev) call per image (n_frames = 1): the status quo
+  (a) mixed     one b200timg_blocks_mixed_dev (sixel pages: b200timg_sixel_mixed_dev, kitty pages:
+                b200timg_graphics_mixed_dev) call for the page
+  (b) per_image one b200timg_blocks_batch_dev (b200timg_sixel_batch_dev, b200timg_graphics_batch_dev) call per image
+                (n_frames = 1): the status quo
   (c) per_geom  one uniform batch call per distinct geometry (sources regrouped by geometry)
   (d) the cost of generality: C3 geometry (1920x1080 -> 320x90, -p quarter, 64 frames) through the mixed call against
       b200timg_blocks_batch_dev, and C4's (3840x2160 -> 337x190, -p sixel, 64 frames) through the sixel mixed call
-      against b200timg_sixel_batch_dev with flags = 0
+      against b200timg_sixel_batch_dev with flags = 0, and C4's through the kitty mixed call (stored and deflate) against
+      b200timg_graphics_batch_dev with flags = 0
 (a), (b) and (c) must produce the same bytes for every image (asserted); so must both sides of (d).  Per-kernel ms of one
 (a) and one (b) page come from b200timg_profile in a separate run.  The GPU's name, power limit and max SM clock are read
 in the same run.
@@ -44,6 +51,10 @@ PAGES = {
     "grid4x4-half": dict(cols=4, rows=4, term=(300, 100), quarter=False),
     "grid4x4-sixel": dict(cols=4, rows=4, term=(300, 100), quarter=False, sixel=True),
     "grid8x8-sixel": dict(cols=8, rows=8, term=(300, 100), quarter=False, sixel=True),
+    "grid8x8-kitty": dict(cols=8, rows=8, term=(300, 100), quarter=False, kitty=True, deflate=False),
+    "grid8x8-kitty-deflate": dict(cols=8, rows=8, term=(300, 100), quarter=False, kitty=True, deflate=True),
+    "grid4x4-kitty": dict(cols=4, rows=4, term=(300, 100), quarter=False, kitty=True, deflate=False),
+    "grid4x4-kitty-deflate": dict(cols=4, rows=4, term=(300, 100), quarter=False, kitty=True, deflate=True),
 }
 
 
@@ -58,7 +69,8 @@ def gpu_info():
 
 def page_layout(cfg):
     """(images' source sizes, fitted outputs, indents) of one page, as timg.cc:938-939 and renderer.cc lay it out."""
-    cx, cy = (9, 18) if cfg.get("sixel") else (2, 2) if cfg["quarter"] else (1, 2)
+    pixels = cfg.get("sixel") or cfg.get("kitty")
+    cx, cy = (9, 18) if pixels else (2, 2) if cfg["quarter"] else (1, 2)
     box_w = cfg["term"][0] * cx // cfg["cols"]
     box_h = cfg["term"][1] * cy // cfg["rows"]
     n = cfg["cols"] * cfg["rows"]
@@ -68,7 +80,7 @@ def page_layout(cfg):
         _, ow, oh = timg_b200.calc_fit(iw, ih, box_w, box_h, cx, cy)
         srcs.append((iw, ih))
         outs.append((ow, oh))
-        indents.append(0 if cfg.get("sixel") else (i % cfg["cols"]) * box_w // cx)   # UnicodeBlockCanvas::Send's x / cell_x_px
+        indents.append(0 if pixels else (i % cfg["cols"]) * box_w // cx)   # UnicodeBlockCanvas::Send's x / cell_x_px
     return srcs, outs, indents
 
 
@@ -101,22 +113,38 @@ def timed(torch, fn, steps):
     return (time.perf_counter() - t0) * 1e3 / steps
 
 
-def encoder(L, sixel):
-    """(mixed call, uniform batch call, per-frame staging bound) of the block or the sixel encoder."""
-    if sixel:
-        return (L.b200timg_sixel_mixed_dev, L.b200timg_sixel_batch_dev,
+def encoder(L, cfg, n):
+    """(mixed call, uniform batch call, per-frame staging bound) of the block, sixel or kitty encoder.  Both calls take
+    (ctx, batch, src, out, cap, offsets); the uniform one also the frames it encodes (kitty: their ids)."""
+    if cfg.get("sixel"):
+        return (L.b200timg_sixel_mixed_dev, lambda *a: L.b200timg_sixel_batch_dev(*a[:6]),
                 lambda ow, oh: L.b200timg_sixel_bound(ow, (oh + 5) // 6 * 6))
-    return L.b200timg_blocks_mixed_dev, L.b200timg_blocks_batch_dev, L.b200timg_blocks_bound
+    if cfg.get("kitty"):                       # -pk, tmux off, rgb24 (timg's default local_alpha_handling), 9 x 18 px cells
+        proto = timg_b200.KITTY | (timg_b200.DEFLATE if cfg["deflate"] else 0)
+        ids = (C.c_uint32 * n)(*range(1, n + 1))
+        page = timg_b200.Graphics(proto, 1, C.cast(ids, C.POINTER(C.c_uint32)), 9, 18, 0)
+        per_call = {}                          # the frames of a uniform call -> its description (built outside the timing)
+
+        def uniform(h, b, src, out, cap, offs, members):
+            key = tuple(members)
+            if key not in per_call:
+                arr = (C.c_uint32 * len(key))(*[ids[i] for i in key])
+                per_call[key] = (timg_b200.Graphics(proto, 1, C.cast(arr, C.POINTER(C.c_uint32)), 9, 18, 0), arr)
+            return L.b200timg_graphics_batch_dev(h, b, C.byref(per_call[key][0]), src, out, cap, offs)
+        bound_g = timg_b200.Graphics(proto, 1, None, 9, 18, 0)
+        return ((lambda h, b, *a, _keep=(ids, page): L.b200timg_graphics_mixed_dev(h, b, C.byref(page), *a)), uniform,
+                lambda ow, oh: L.b200timg_graphics_size(C.byref(bound_g), ow, oh, 0xFFFFFFFF))
+    return L.b200timg_blocks_mixed_dev, lambda *a: L.b200timg_blocks_batch_dev(*a[:6]), L.b200timg_blocks_bound
 
 
 def run_page(name, cfg, steps, warmup, torch):
     L = timg_b200.lib()
     ctx = timg_b200.Context(0)
-    mixed_fn, batch_fn, bound_fn = encoder(L, cfg.get("sixel", False))
     flags = timg_b200.QUARTER if cfg["quarter"] else 0
     bg = timg_b200.rgba_u32(0, 0, 0)
     srcs, outs, indents = page_layout(cfg)
     n = len(srcs)
+    mixed_fn, batch_fn, bound_fn = encoder(L, cfg, n)
     imgs = device_images(torch, srcs)
     flat, offs = pack(torch, imgs)
     torch.cuda.synchronize()                   # sources are written on torch's stream, read on the context's
@@ -142,7 +170,7 @@ def run_page(name, cfg, steps, warmup, torch):
     def run_b():
         for i in range(n):
             ctx._chk(batch_fn(ctx.h, C.byref(b_batches[i]), flat.data_ptr() + offs[i],
-                              d_out_b.data_ptr() + int(slot[i]), bounds[i], d_offs_b[i].data_ptr()))
+                              d_out_b.data_ptr() + int(slot[i]), bounds[i], d_offs_b[i].data_ptr(), [i]))
 
     # (c): images regrouped by geometry; one uniform call per geometry (the indent is per call, so frames of a group
     # that sit in different columns would need one call each: the bytes are compared with indents folded in below)
@@ -163,8 +191,9 @@ def run_page(name, cfg, steps, warmup, torch):
     c_base = np.cumsum([0] + [c[2] for c in c_calls])
 
     def run_c():
-        for j, (b, o, gcap, d_o, _) in enumerate(c_calls):
-            ctx._chk(batch_fn(ctx.h, C.byref(b), flat_c.data_ptr() + o, d_out_c.data_ptr() + int(c_base[j]), gcap, d_o.data_ptr()))
+        for j, (b, o, gcap, d_o, members) in enumerate(c_calls):
+            ctx._chk(batch_fn(ctx.h, C.byref(b), flat_c.data_ptr() + o, d_out_c.data_ptr() + int(c_base[j]), gcap, d_o.data_ptr(),
+                              members))
 
     for _ in range(warmup):
         run_a(); run_b(); run_c()
@@ -214,6 +243,8 @@ def run_page(name, cfg, steps, warmup, torch):
 GENERALITY = {
     "C3-generality": dict(iw=1920, ih=1080, ow=320, oh=90, flags=timg_b200.QUARTER, sixel=False),
     "C4-generality": dict(iw=3840, ih=2160, ow=337, oh=190, flags=0, sixel=True),
+    "C4-kitty-generality": dict(iw=3840, ih=2160, ow=337, oh=190, flags=0, kitty=True, deflate=False),
+    "C4-kitty-deflate-generality": dict(iw=3840, ih=2160, ow=337, oh=190, flags=0, kitty=True, deflate=True),
 }
 
 
@@ -221,7 +252,7 @@ def run_generality(name, g, steps, warmup, torch):
     """(d): one geometry through the mixed call and through the uniform batch."""
     L = timg_b200.lib()
     ctx = timg_b200.Context(0)
-    mixed_fn, batch_fn, bound_fn = encoder(L, g["sixel"])
+    mixed_fn, batch_fn, bound_fn = encoder(L, g, 64)
     n, iw, ih, ow, oh, indent, flags = 64, g["iw"], g["ih"], g["ow"], g["oh"], 0, g["flags"]
     bg = timg_b200.rgba_u32(0, 0, 0)
     base = synth.frame_torch(800, iw, ih, "photo")
@@ -243,7 +274,7 @@ def run_generality(name, g, steps, warmup, torch):
         ctx._chk(mixed_fn(ctx.h, C.byref(mb), d_src.data_ptr(), outs[0].data_ptr(), cap, offs[0].data_ptr()))
 
     def uniform():
-        ctx._chk(batch_fn(ctx.h, C.byref(ub), d_src.data_ptr(), outs[1].data_ptr(), cap, offs[1].data_ptr()))
+        ctx._chk(batch_fn(ctx.h, C.byref(ub), d_src.data_ptr(), outs[1].data_ptr(), cap, offs[1].data_ptr(), list(range(n))))
     for _ in range(warmup):
         mixed(); uniform()
     tm = tu = 0.0
