@@ -420,6 +420,30 @@ int b200timg_windows(b200timg_ctx *ctx, const uint8_t *img, int w, int h, int dw
 int b200timg_windows_dev(b200timg_ctx *ctx, const uint8_t *d_img, int w, int h, int dw, int dh, long long x0,
                          long long y0, int dx, int dy, long long first_pos, int n_pos, uint8_t *d_out);
 
+/* ======================= animated GIFs: the STB source's decode (SURVEY 8f rank 4) ===================
+ * Frame k's canvas is the RGBA buffer the k-th call of stbi__gif_load_next(ctx, g, comp, 4, two_back = NULL) returns
+ * (third_party/stb/stb_image.h:6779-6951), as src/stb-image-source.cc:120-140 loops over it: dispose 3 acts as 2,
+ * bytes past the end of the file read as 0, and the loop stops at the terminator or at the first error.
+ *
+ * Host only: stbi__gif_load_next's block walk without decoding rasters (two_back = NULL). *w, *h: the logical
+ * screen; *n_frames: frames up to the terminator or the first error the walk can see; delays_ms[k] (first
+ * delays_cap entries, may be NULL): gdata.delay after frame k.  B200TIMG_EINVAL: not GIF87a/89a ("not a GIF", so an
+ * adapter can fall through to the next source), no frame, a zero-sized screen. */
+int b200timg_gif_parse(const uint8_t *gif, size_t size, int *w, int *h, int *n_frames, int32_t *delays_ms,
+                       int delays_cap);
+/* Canvases of frames 0..n_frames-1, RGBA w*h*4 each, back to back: the source layout of a b200timg_batch with
+ * src_w = w, src_h = h, src_fmt = B200TIMG_FMT_RGBA.  gif: HOST bytes, uploaded through context-owned pinned
+ * staging; the call does not wait for its own work, but before it rewrites the staging it waits on the host for the
+ * previous call's upload to finish (that copy runs in stream order, after whatever the stream held before it).  *d_valid (device): the frames the reference's loop collects
+ * (LZW errors are found on the device); canvases from there on are written, in bounds, with unspecified contents.
+ * d_frames and d_valid must be 4-byte aligned (B200TIMG_EINVAL otherwise).  n_frames <= what b200timg_gif_parse
+ * reports.  A call launches three kernels whatever n_frames is. */
+int b200timg_gif_frames_dev(b200timg_ctx *ctx, const uint8_t *gif, size_t size, int n_frames, uint8_t *d_frames,
+                            int32_t *d_valid);
+/* Host form: frames gets n_frames * w*h*4 bytes, *n_valid the frames the reference collects. */
+int b200timg_gif_frames(b200timg_ctx *ctx, const uint8_t *gif, size_t size, int n_frames, uint8_t *frames,
+                        int *n_valid);
+
 /* ======================= Kitty / iTerm2 canvases: PNG + base64 (SURVEY 8f rank 2) ===================
  * png::Encode (src/timg-png.cc:90-152): signature, IHDR, one IDAT holding the zlib stream of the scanlines (each
  * row filtered with "Sub"), IEND.  rgb24 != 0: colour type 2 (png::ColorEncoding::kRGB_24), else RGBA.  The

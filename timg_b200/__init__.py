@@ -158,6 +158,10 @@ ABI = {
                                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     "b200timg_sixel_shape_of": (C.c_int, [C.c_int] * 5 + [C.POINTER(SixelShape)]),
     "b200timg_scale_shape_of": (C.c_int, [C.c_int] * 8 + [C.POINTER(ScaleShape)]),
+    "b200timg_gif_parse": (C.c_int, [C.c_void_p, C.c_size_t, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int),
+                                     C.c_void_p, C.c_int]),
+    "b200timg_gif_frames_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_void_p]),
+    "b200timg_gif_frames": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.POINTER(C.c_int)]),
 }
 
 _lib = None
@@ -259,6 +263,20 @@ def graphics_size(protocol, w, h, rgb24=False, id=0, cell=None, indent=0):
     """Exact bytes of one framed kitty / iTerm2 frame (host only); 0 for invalid arguments."""
     g, _ = graphics(protocol, rgb24, cell=cell, indent=indent)
     return lib().b200timg_graphics_size(C.byref(g), w, h, id)
+
+
+def gif_parse(data):
+    """b200timg_gif_parse (host only): (w, h, delays_ms) of a GIF, one delay per frame the STB source collects unless
+    an LZW error (found only by decoding) ends the animation earlier.  Raises B200Error(EINVAL) for what is not a
+    GIF87a / GIF89a, has no frame or a zero-sized screen."""
+    data = bytes(data)
+    w, h, n = C.c_int(), C.c_int(), C.c_int()
+    rc = lib().b200timg_gif_parse(data, len(data), C.byref(w), C.byref(h), C.byref(n), None, 0)
+    if rc != OK:
+        raise B200Error(rc, "gif_parse: not a GIF, no frame or a zero-sized screen")
+    delays = np.zeros(max(1, n.value), np.int32)
+    lib().b200timg_gif_parse(data, len(data), C.byref(w), C.byref(h), C.byref(n), delays.ctypes.data, n.value)
+    return w.value, h.value, [int(d) for d in delays[:n.value]]
 
 
 def _np_ptr(a):
@@ -594,6 +612,29 @@ class Context:
         self._chk(lib().b200timg_graphics_batch_dev(self.h, C.byref(b), C.byref(g), d_src.data_ptr(), d_out.data_ptr(),
                                                     out_cap, d_offsets.data_ptr()))
         return d_out, d_offsets
+
+    def gif_frames(self, data, n=None):
+        """b200timg_gif_frames: (canvases [n, h, w, 4] uint8, n_valid) of a GIF's first n frames (default: every frame
+        gif_parse reports); canvases from n_valid on are unspecified."""
+        data = bytes(data)
+        w, h, delays = gif_parse(data)
+        n = len(delays) if n is None else n
+        out = np.empty((max(1, n), h, w, 4), np.uint8)
+        valid = C.c_int()
+        self._chk(lib().b200timg_gif_frames(self.h, data, len(data), n, out.ctypes.data, C.byref(valid)))
+        return out[:n], valid.value
+
+    def gif_frames_dev(self, data, d_frames, n):
+        """b200timg_gif_frames_dev into a device tensor of at least n * h * w * 4 bytes (the source of a uniform batch):
+        returns d_valid, a one-element int32 device tensor, after the (asynchronous) call."""
+        import torch
+        data = bytes(data)
+        w, h, _ = gif_parse(data)
+        if d_frames.numel() * d_frames.element_size() < n * w * h * 4:
+            raise B200Error(EINVAL, f"gif_frames_dev: d_frames holds fewer than {n} canvases of {w}x{h}")
+        d_valid = torch.empty(1, dtype=torch.int32, device=d_frames.device)
+        self._chk(lib().b200timg_gif_frames_dev(self.h, data, len(data), n, d_frames.data_ptr(), d_valid.data_ptr()))
+        return d_valid
 
     @staticmethod
     def graphics_mixed_bound(b, g):

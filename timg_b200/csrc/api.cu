@@ -76,6 +76,8 @@ void b200timg_ctx_destroy(b200timg_ctx *ctx) {
     ctx->tables.release(); ctx->sixel_work.release(); ctx->misc.release(); ctx->scale_list.release(); ctx->scale_tmp.release(); ctx->tri_tables.release();
     ctx->mixed_arena.release(); ctx->mixed_stage.release();
     if (ctx->ev_mixed) cudaEventDestroy(ctx->ev_mixed);
+    ctx->gif_arena.release(); ctx->gif_scratch.release(); ctx->gif_stage.release();
+    if (ctx->ev_gif) cudaEventDestroy(ctx->ev_gif);
     ctx->pinned.release(); ctx->pinned_io.release();
     ctx->png_sums.release(); ctx->gfx_ids.release();
     ctx->dfl_raw.release(); ctx->dfl_scratch.release(); ctx->dfl_meta.release(); ctx->dfl_tokens.release(); ctx->dfl_png.release();

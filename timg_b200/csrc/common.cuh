@@ -124,6 +124,11 @@ struct b200timg_ctx {
     b200timg::DevBuf mixed_arena;
     b200timg::HostBuf mixed_stage;
     cudaEvent_t ev_mixed = nullptr;
+    // GIF decode (gif.cu): file + frame descriptors uploaded in one copy from gif_stage (rewritten once ev_gif says the
+    // previous call's copy has run), and the call's code streams, index planes and per-frame reach
+    b200timg::DevBuf gif_arena, gif_scratch;
+    b200timg::HostBuf gif_stage;
+    cudaEvent_t ev_gif = nullptr;
 
     int fail(int code, const char *fmt, ...) {
         va_list ap; va_start(ap, fmt);
