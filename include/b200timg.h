@@ -444,6 +444,39 @@ int b200timg_gif_frames_dev(b200timg_ctx *ctx, const uint8_t *gif, size_t size, 
 int b200timg_gif_frames(b200timg_ctx *ctx, const uint8_t *gif, size_t size, int n_frames, uint8_t *frames,
                         int *n_valid);
 
+/* ======================= baseline JPEGs: the STB source's decode (SURVEY 8f rank 4) ===================
+ * File f's canvas is the w*h*4 RGBA buffer stbi__load_and_postprocess_8bit(ctx, &w, &h, &c, 4) returns for it on
+ * x86-64 (SSE2 IDCT, colour conversion and hv_2 resampler), which is what src/stb-image-source.cc:141-157 scales.
+ *
+ * Host only: stb's marker walk (stbi__decode_jpeg_header / stbi__decode_jpeg_image) without entropy decoding.
+ * B200TIMG_EINVAL where that walk fails (no SOI, bad SOF, bad DQT / DHT before SOF, bad SOS, bad DNL, ...), so the
+ * reference's source fails too.  supported = 0 (reason says why) for what the device does not take: progressive
+ * files, more than one scan, a scan without every component, an undefined Huffman table, and files whose reference
+ * result is uninitialised memory because no scan is decoded before the walk stops. */
+typedef struct {
+    int w, h, n_comp;
+    int h_samp[4], v_samp[4];      /* sampling factors of components 0..n_comp-1 */
+    int restart_interval;          /* DRI in force at the scan, 0 if none */
+    int progressive;
+    int supported;
+    char reason[96];
+} b200timg_jpeg_info;
+int b200timg_jpeg_parse(const uint8_t *jpg, size_t size, b200timg_jpeg_info *info);
+/* Canvases of n_files files back to back: file f at d_frames + sum_{g<f} w_g*h_g*4, the src_offset layout of a
+ * b200timg_mixed_batch with B200TIMG_FMT_RGBA.  files: HOST bytes, uploaded in one copy through context-owned pinned
+ * staging (the call waits on the host for the previous call's upload before it rewrites the staging, never for its
+ * own work).  d_status[f] (device): 1 the canvas is the reference's; 0 stb returns NULL (a Huffman code or DC error
+ * on the decode path), the canvas is unspecified; -1 the file bails at a restart boundary (stb returns success with
+ * the rest of its planes uninitialised), so the caller decodes it on the CPU.  B200TIMG_EINVAL before any launch,
+ * naming the file: a file b200timg_jpeg_parse rejects or reports unsupported, n_files <= 0, d_frames or d_status not
+ * 4-byte aligned.  A call launches seven kernels whatever n_files is; the decoder's synchronisation rounds run
+ * inside them. */
+int b200timg_jpeg_frames_dev(b200timg_ctx *ctx, int n_files, const uint8_t *const *files, const size_t *sizes,
+                             uint8_t *d_frames, int32_t *d_status);
+/* Host form: frames gets the canvases back to back, status[f] as above. */
+int b200timg_jpeg_frames(b200timg_ctx *ctx, int n_files, const uint8_t *const *files, const size_t *sizes,
+                         uint8_t *frames, int32_t *status);
+
 /* ======================= Kitty / iTerm2 canvases: PNG + base64 (SURVEY 8f rank 2) ===================
  * png::Encode (src/timg-png.cc:90-152): signature, IHDR, one IDAT holding the zlib stream of the scanlines (each
  * row filtered with "Sub"), IEND.  rgb24 != 0: colour type 2 (png::ColorEncoding::kRGB_24), else RGBA.  The

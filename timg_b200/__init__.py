@@ -162,6 +162,9 @@ ABI = {
                                      C.c_void_p, C.c_int]),
     "b200timg_gif_frames_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_void_p]),
     "b200timg_gif_frames": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.POINTER(C.c_int)]),
+    "b200timg_jpeg_parse": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200timg_jpeg_frames_dev": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200timg_jpeg_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 _lib = None
@@ -277,6 +280,33 @@ def gif_parse(data):
     delays = np.zeros(max(1, n.value), np.int32)
     lib().b200timg_gif_parse(data, len(data), C.byref(w), C.byref(h), C.byref(n), delays.ctypes.data, n.value)
     return w.value, h.value, [int(d) for d in delays[:n.value]]
+
+
+class JpegInfo(C.Structure):
+    _fields_ = [("w", C.c_int), ("h", C.c_int), ("n_comp", C.c_int), ("h_samp", C.c_int * 4), ("v_samp", C.c_int * 4),
+                ("restart_interval", C.c_int), ("progressive", C.c_int), ("supported", C.c_int),
+                ("reason", C.c_char * 96)]
+
+
+def jpeg_parse(data):
+    """b200timg_jpeg_parse (host only): a dict of w, h, n_comp, h_samp, v_samp, restart_interval, progressive,
+    supported and reason.  Raises B200Error(EINVAL) where stb's marker walk fails (so the reference's source fails)."""
+    data = bytes(data)
+    info = JpegInfo()
+    rc = lib().b200timg_jpeg_parse(data, len(data), C.byref(info))
+    if rc != OK:
+        raise B200Error(rc, "jpeg_parse: stb's JPEG header walk fails")
+    n = info.n_comp
+    return dict(w=info.w, h=info.h, n_comp=n, h_samp=list(info.h_samp[:n]), v_samp=list(info.v_samp[:n]),
+                restart_interval=info.restart_interval, progressive=bool(info.progressive),
+                supported=bool(info.supported), reason=info.reason.decode())
+
+
+def _jpeg_args(files):
+    files = [bytes(f) for f in files]
+    bufs = (C.c_char_p * len(files))(*files)
+    sizes = (C.c_size_t * len(files))(*[len(f) for f in files])
+    return files, bufs, sizes
 
 
 def _np_ptr(a):
@@ -635,6 +665,30 @@ class Context:
         d_valid = torch.empty(1, dtype=torch.int32, device=d_frames.device)
         self._chk(lib().b200timg_gif_frames_dev(self.h, data, len(data), n, d_frames.data_ptr(), d_valid.data_ptr()))
         return d_valid
+
+    def jpeg_frames(self, files):
+        """b200timg_jpeg_frames: (list of [h, w, 4] uint8 canvases, int32 status per file) for a list of JPEG files."""
+        files, bufs, sizes = _jpeg_args(files)
+        geo = [jpeg_parse(f) for f in files] if files else []
+        total = sum(g["w"] * g["h"] * 4 for g in geo)
+        out = np.empty(max(1, total), np.uint8)
+        status = np.zeros(max(1, len(files)), np.int32)
+        self._chk(lib().b200timg_jpeg_frames(self.h, len(files), bufs, sizes, out.ctypes.data, status.ctypes.data))
+        canv, o = [], 0
+        for g in geo:
+            canv.append(out[o:o + g["w"] * g["h"] * 4].reshape(g["h"], g["w"], 4))
+            o += g["w"] * g["h"] * 4
+        return canv, status[:len(files)]
+
+    def jpeg_frames_dev(self, files, d_frames, d_status=None):
+        """b200timg_jpeg_frames_dev into a device tensor holding every canvas back to back (the src_offset layout of a
+        mixed batch): returns d_status, an int32 device tensor with one entry per file, after the (asynchronous) call."""
+        import torch
+        files, bufs, sizes = _jpeg_args(files)
+        if d_status is None:
+            d_status = torch.empty(max(1, len(files)), dtype=torch.int32, device=d_frames.device)
+        self._chk(lib().b200timg_jpeg_frames_dev(self.h, len(files), bufs, sizes, d_frames.data_ptr(), d_status.data_ptr()))
+        return d_status
 
     @staticmethod
     def graphics_mixed_bound(b, g):

@@ -129,6 +129,11 @@ struct b200timg_ctx {
     b200timg::DevBuf gif_arena, gif_scratch;
     b200timg::HostBuf gif_stage;
     cudaEvent_t ev_gif = nullptr;
+    // JPEG decode (jpeg.cu): files + descriptors + Huffman tables uploaded in one copy from jpeg_stage (rewritten once
+    // ev_jpeg says the previous call's copy has run), and the call's streams, decoder states, coefficients and planes
+    b200timg::DevBuf jpeg_arena, jpeg_scratch;
+    b200timg::HostBuf jpeg_stage;
+    cudaEvent_t ev_jpeg = nullptr;
 
     int fail(int code, const char *fmt, ...) {
         va_list ap; va_start(ap, fmt);
