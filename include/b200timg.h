@@ -477,6 +477,48 @@ int b200timg_jpeg_frames_dev(b200timg_ctx *ctx, int n_files, const uint8_t *cons
 int b200timg_jpeg_frames(b200timg_ctx *ctx, int n_files, const uint8_t *const *files, const size_t *sizes,
                          uint8_t *frames, int32_t *status);
 
+/* ======================= PNG files: the STB source's decode ===================
+ * File f's canvas is the w*h*4 RGBA buffer stbi__load_and_postprocess_8bit(ctx, &w, &h, &c, 4) returns for it, which
+ * is what src/stb-image-source.cc:141-157 scales: stb's chunk walk, zlib reader, unfiltering, Adam7, tRNS, palette
+ * expansion and 16->8 reduction, quirks included (no CRC or Adler-32 check, bytes past the end read as 0, the whole
+ * zlib stream decoded up to its final block).
+ *
+ * Host only: stb's chunk walk (stbi__parse_png_file) without inflating.  B200TIMG_EINVAL where that walk fails (no PNG
+ * signature, a bad or second IHDR, a bad PLTE or tRNS, an unknown critical chunk, no IDAT, no IEND before the data
+ * ends, ...), so the reference's source fails too and an adapter can try the next source.  apng: an acTL among the
+ * chunk headers in the first 1024 bytes (HasAPNGHeader, src/image-source.cc:297-326), the test LooksLikeAPNG makes in
+ * video builds; the device decodes the default image, as the STB source does.  supported = 0 (reason says why) for
+ * what the device does not take: more than 2^31 raw (filtered) bytes, a canvas of more than 2^31 bytes, 2^31 IDAT
+ * bytes or more, a skipped chunk of 2^31 bytes or more, and an initial inflate buffer size stb computes as a
+ * non-positive int.  A skipped chunk of 2^31 bytes or more ends the walk: stb's skip takes an int, and a negative one
+ * moves it to the end of its read buffer, so what it reads next depends on how the file is read, not on the file;
+ * the fields are those read up to that chunk (w and h are 0 if it comes before IHDR). */
+typedef struct {
+    int w, h, bit_depth, color_type, interlace;
+    int palette_len;               /* entries of the PLTE in force, 0 if none */
+    int trns;                      /* 0 none, 1 palette alpha, 2 grey / RGB colour key */
+    int cgbi;                      /* a CgBI chunk: the IDATs hold a raw deflate stream (no zlib header) */
+    int apng;
+    unsigned long long idat_bytes; /* the IDAT payloads, joined */
+    int supported;
+    char reason[96];
+} b200timg_png_info;
+int b200timg_png_parse(const uint8_t *png, size_t size, b200timg_png_info *info);
+/* Canvases of n_files files back to back: file f at d_frames + sum_{g<f} w_g*h_g*4, the src_offset layout of a
+ * b200timg_mixed_batch with B200TIMG_FMT_RGBA.  files: HOST bytes, uploaded in one copy through context-owned pinned
+ * staging (the call waits on the host for the previous call's upload before it rewrites the staging, never for its
+ * own work).  d_status[f] (device): 1 the canvas is the reference's; 0 stb returns NULL (a zlib error, too little
+ * data, a bad filter type), the canvas is unspecified; -1 a palette index past the entries stb has written, so the
+ * reference canvas is uninitialised memory and the caller decodes the file on the CPU (0 takes precedence).
+ * B200TIMG_EINVAL before any launch, naming the file: a file b200timg_png_parse rejects or reports unsupported,
+ * n_files <= 0, d_frames or d_status not 4-byte aligned, 2^32 raw bytes or more in one call.  A call launches 38
+ * kernels whatever n_files is and whatever the files hold. */
+int b200timg_png_frames_dev(b200timg_ctx *ctx, int n_files, const uint8_t *const *files, const size_t *sizes,
+                            uint8_t *d_frames, int32_t *d_status);
+/* Host form: frames gets the canvases back to back, status[f] as above. */
+int b200timg_png_frames(b200timg_ctx *ctx, int n_files, const uint8_t *const *files, const size_t *sizes,
+                        uint8_t *frames, int32_t *status);
+
 /* ======================= Kitty / iTerm2 canvases: PNG + base64 (SURVEY 8f rank 2) ===================
  * png::Encode (src/timg-png.cc:90-152): signature, IHDR, one IDAT holding the zlib stream of the scanlines (each
  * row filtered with "Sub"), IEND.  rgb24 != 0: colour type 2 (png::ColorEncoding::kRGB_24), else RGBA.  The

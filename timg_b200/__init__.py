@@ -165,6 +165,9 @@ ABI = {
     "b200timg_jpeg_parse": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200timg_jpeg_frames_dev": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200timg_jpeg_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200timg_png_parse": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200timg_png_frames_dev": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200timg_png_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 _lib = None
@@ -300,6 +303,26 @@ def jpeg_parse(data):
     return dict(w=info.w, h=info.h, n_comp=n, h_samp=list(info.h_samp[:n]), v_samp=list(info.v_samp[:n]),
                 restart_interval=info.restart_interval, progressive=bool(info.progressive),
                 supported=bool(info.supported), reason=info.reason.decode())
+
+
+class PngInfo(C.Structure):
+    _fields_ = [("w", C.c_int), ("h", C.c_int), ("bit_depth", C.c_int), ("color_type", C.c_int), ("interlace", C.c_int),
+                ("palette_len", C.c_int), ("trns", C.c_int), ("cgbi", C.c_int), ("apng", C.c_int),
+                ("idat_bytes", C.c_ulonglong), ("supported", C.c_int), ("reason", C.c_char * 96)]
+
+
+def png_parse(data):
+    """b200timg_png_parse (host only): a dict of w, h, bit_depth, color_type, interlace, palette_len, trns (0 none,
+    1 palette alpha, 2 colour key), cgbi, apng, idat_bytes, supported and reason.  Raises B200Error(EINVAL) where stb's
+    chunk walk fails (so the reference's source fails), a non-PNG file included."""
+    data = bytes(data)
+    info = PngInfo()
+    rc = lib().b200timg_png_parse(data, len(data), C.byref(info))
+    if rc != OK:
+        raise B200Error(rc, "png_parse: stb's PNG chunk walk fails")
+    return dict(w=info.w, h=info.h, bit_depth=info.bit_depth, color_type=info.color_type, interlace=info.interlace,
+                palette_len=info.palette_len, trns=info.trns, cgbi=bool(info.cgbi), apng=bool(info.apng),
+                idat_bytes=info.idat_bytes, supported=bool(info.supported), reason=info.reason.decode())
 
 
 def _jpeg_args(files):
@@ -688,6 +711,30 @@ class Context:
         if d_status is None:
             d_status = torch.empty(max(1, len(files)), dtype=torch.int32, device=d_frames.device)
         self._chk(lib().b200timg_jpeg_frames_dev(self.h, len(files), bufs, sizes, d_frames.data_ptr(), d_status.data_ptr()))
+        return d_status
+
+    def png_frames(self, files):
+        """b200timg_png_frames: (list of [h, w, 4] uint8 canvases, int32 status per file) for a list of PNG files."""
+        files, bufs, sizes = _jpeg_args(files)
+        geo = [png_parse(f) for f in files] if files else []
+        total = sum(g["w"] * g["h"] * 4 for g in geo)
+        out = np.empty(max(1, total), np.uint8)
+        status = np.zeros(max(1, len(files)), np.int32)
+        self._chk(lib().b200timg_png_frames(self.h, len(files), bufs, sizes, out.ctypes.data, status.ctypes.data))
+        canv, o = [], 0
+        for g in geo:
+            canv.append(out[o:o + g["w"] * g["h"] * 4].reshape(g["h"], g["w"], 4))
+            o += g["w"] * g["h"] * 4
+        return canv, status[:len(files)]
+
+    def png_frames_dev(self, files, d_frames, d_status=None):
+        """b200timg_png_frames_dev into a device tensor holding every canvas back to back (the src_offset layout of a
+        mixed batch): returns d_status, an int32 device tensor with one entry per file, after the (asynchronous) call."""
+        import torch
+        files, bufs, sizes = _jpeg_args(files)
+        if d_status is None:
+            d_status = torch.empty(max(1, len(files)), dtype=torch.int32, device=d_frames.device)
+        self._chk(lib().b200timg_png_frames_dev(self.h, len(files), bufs, sizes, d_frames.data_ptr(), d_status.data_ptr()))
         return d_status
 
     @staticmethod

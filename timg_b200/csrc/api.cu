@@ -80,6 +80,8 @@ void b200timg_ctx_destroy(b200timg_ctx *ctx) {
     if (ctx->ev_gif) cudaEventDestroy(ctx->ev_gif);
     ctx->jpeg_arena.release(); ctx->jpeg_scratch.release(); ctx->jpeg_stage.release();
     if (ctx->ev_jpeg) cudaEventDestroy(ctx->ev_jpeg);
+    ctx->png_arena.release(); ctx->png_scratch.release(); ctx->png_stage.release();
+    if (ctx->ev_png) cudaEventDestroy(ctx->ev_png);
     ctx->pinned.release(); ctx->pinned_io.release();
     ctx->png_sums.release(); ctx->gfx_ids.release();
     ctx->dfl_raw.release(); ctx->dfl_scratch.release(); ctx->dfl_meta.release(); ctx->dfl_tokens.release(); ctx->dfl_png.release();

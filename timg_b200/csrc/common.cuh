@@ -134,6 +134,11 @@ struct b200timg_ctx {
     b200timg::DevBuf jpeg_arena, jpeg_scratch;
     b200timg::HostBuf jpeg_stage;
     cudaEvent_t ev_jpeg = nullptr;
+    // PNG decode (png_decode.cu): files + descriptors uploaded in one copy from png_stage (rewritten once ev_png says
+    // the previous call's copy has run), and the call's zlib streams, raw planes, source indices and copy records
+    b200timg::DevBuf png_arena, png_scratch;
+    b200timg::HostBuf png_stage;
+    cudaEvent_t ev_png = nullptr;
 
     int fail(int code, const char *fmt, ...) {
         va_list ap; va_start(ap, fmt);

@@ -1,0 +1,92 @@
+"""Device PNG decode (b200timg_png_frames_dev) against the reference's STB source on one host core.
+
+Device time: two CUDA events on the context's stream (also torch's current stream) around the call, recorded after a
+device synchronise, so the upload of the files from pinned staging and every kernel are inside it; the per-kernel split
+comes from ctx.profile in a separate call (png_jump_kernel summed over its rounds).  Reference time: the door onto the
+unmodified STBImageSource
+(oracle/gif.mk) at capture=0, one decode per file, on the calling thread.  Prints one JSON line per case with the card's
+name and power limit read in the same run."""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import tempfile
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
+
+import numpy as np  # noqa: E402
+
+import png_cases as pc  # noqa: E402
+import timg_b200  # noqa: E402
+from oracle import gif as G  # noqa: E402
+
+
+def cases():
+    yield "4k_photo_rgb", [pc.pillow(pc.photo(3840, 2160, 1), "RGB")]
+    yield "4k_screenshot_l9", [pc.pillow(pc.screenshot(3840, 2160, 2), "RGB", compress_level=9)]
+    yield "grid64_1080p", [pc.pillow(pc.photo(1920 - 8 * (k % 5), 1080 - 4 * (k % 7), k), "RGB") for k in range(64)]
+    yield "thumbs1024_480x270", [pc.pillow(pc.photo(480, 270, k % 16), "RGB") for k in range(1024)]
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--ref-steps", type=int, default=1)
+    a = ap.parse_args()
+    import torch
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                          capture_output=True, text=True).stdout.strip()
+    stream = torch.cuda.Stream()                               # a real stream that the context launches on
+    ctx = timg_b200.Context(0, stream=stream.cuda_stream)
+    torch.cuda.set_stream(stream)
+    for name, files in cases():
+        geo = [timg_b200.png_parse(f) for f in files]
+        rgba = sum(g["w"] * g["h"] * 4 for g in geo)
+        d = torch.empty(rgba, dtype=torch.uint8, device="cuda:0")
+        for _ in range(a.warmup):
+            ctx.png_frames_dev(files, d)
+        torch.cuda.synchronize()
+        ts = []
+        for _ in range(a.steps):
+            torch.cuda.synchronize()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(stream)
+            st = ctx.png_frames_dev(files, d)
+            e1.record(stream)
+            torch.cuda.synchronize()
+            ts.append(e0.elapsed_time(e1) / 1e3)
+        status = st.cpu().numpy()
+        ctx.profile(True)
+        ctx.png_frames_dev(files, d)
+        torch.cuda.synchronize()
+        prof = {k: round(v[1], 3) for k, v in ctx.profile_report().items() if k.startswith("png_")}
+        ctx.profile(False)
+        ref_ms = None
+        if G.have_ref():
+            with tempfile.TemporaryDirectory() as td:
+                paths = []
+                for i, f in enumerate(files):
+                    p = os.path.join(td, f"{i}.png")
+                    open(p, "wb").write(f)
+                    paths.append(p)
+                rt = []
+                for _ in range(a.ref_steps):
+                    t0 = time.perf_counter()
+                    for p in paths:
+                        G.ref_stb_gif_path(p, capture=False)
+                    rt.append(time.perf_counter() - t0)
+                ref_ms = 1e3 * float(np.median(rt))
+        dev_ms = 1e3 * float(np.median(ts))
+        print(json.dumps(dict(case=name, files=len(files), upload_bytes=sum(len(f) for f in files), rgba_bytes=rgba,
+                              device_ms=round(dev_ms, 3), kernels_ms=prof, ref_one_core_ms=None if ref_ms is None else round(ref_ms, 1),
+                              speedup=None if ref_ms is None else round(ref_ms / dev_ms, 2),
+                              status_ok=int((status == 1).sum()), card=card)), flush=True)
+    ctx.close()
+
+
+if __name__ == "__main__":
+    main()
