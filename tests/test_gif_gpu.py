@@ -119,6 +119,7 @@ def _decode_dev(ctx, data):
     n = len(delays)
     d = torch.empty(n * h * w * 4, dtype=torch.uint8, device=_dev())
     d_valid = ctx.gif_frames_dev(data, d, n)
+    timg_b200.device_sync(torch)                   # d_valid is read on torch's stream, the call ran on the context's
     return d, int(d_valid.cpu()[0]), w, h
 
 

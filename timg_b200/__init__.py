@@ -325,7 +325,7 @@ def png_parse(data):
                 idat_bytes=info.idat_bytes, supported=bool(info.supported), reason=info.reason.decode())
 
 
-def _jpeg_args(files):
+def _file_args(files):
     files = [bytes(f) for f in files]
     bufs = (C.c_char_p * len(files))(*files)
     sizes = (C.c_size_t * len(files))(*[len(f) for f in files])
@@ -689,53 +689,46 @@ class Context:
         self._chk(lib().b200timg_gif_frames_dev(self.h, data, len(data), n, d_frames.data_ptr(), d_valid.data_ptr()))
         return d_valid
 
-    def jpeg_frames(self, files):
-        """b200timg_jpeg_frames: (list of [h, w, 4] uint8 canvases, int32 status per file) for a list of JPEG files."""
-        files, bufs, sizes = _jpeg_args(files)
-        geo = [jpeg_parse(f) for f in files] if files else []
+    def _files_frames(self, fn, parse, files):
+        """The host form of a multi-file decode (jpeg_frames, png_frames); parse gives each file's w and h."""
+        files, bufs, sizes = _file_args(files)
+        geo = [parse(f) for f in files]
         total = sum(g["w"] * g["h"] * 4 for g in geo)
         out = np.empty(max(1, total), np.uint8)
         status = np.zeros(max(1, len(files)), np.int32)
-        self._chk(lib().b200timg_jpeg_frames(self.h, len(files), bufs, sizes, out.ctypes.data, status.ctypes.data))
+        self._chk(fn(self.h, len(files), bufs, sizes, out.ctypes.data, status.ctypes.data))
         canv, o = [], 0
         for g in geo:
             canv.append(out[o:o + g["w"] * g["h"] * 4].reshape(g["h"], g["w"], 4))
             o += g["w"] * g["h"] * 4
         return canv, status[:len(files)]
+
+    def _files_frames_dev(self, fn, files, d_frames, d_status):
+        """The dev form of a multi-file decode (jpeg_frames_dev, png_frames_dev)."""
+        import torch
+        files, bufs, sizes = _file_args(files)
+        if d_status is None:
+            d_status = torch.empty(max(1, len(files)), dtype=torch.int32, device=d_frames.device)
+        self._chk(fn(self.h, len(files), bufs, sizes, d_frames.data_ptr(), d_status.data_ptr()))
+        return d_status
+
+    def jpeg_frames(self, files):
+        """b200timg_jpeg_frames: (list of [h, w, 4] uint8 canvases, int32 status per file) for a list of JPEG files."""
+        return self._files_frames(lib().b200timg_jpeg_frames, jpeg_parse, files)
 
     def jpeg_frames_dev(self, files, d_frames, d_status=None):
         """b200timg_jpeg_frames_dev into a device tensor holding every canvas back to back (the src_offset layout of a
         mixed batch): returns d_status, an int32 device tensor with one entry per file, after the (asynchronous) call."""
-        import torch
-        files, bufs, sizes = _jpeg_args(files)
-        if d_status is None:
-            d_status = torch.empty(max(1, len(files)), dtype=torch.int32, device=d_frames.device)
-        self._chk(lib().b200timg_jpeg_frames_dev(self.h, len(files), bufs, sizes, d_frames.data_ptr(), d_status.data_ptr()))
-        return d_status
+        return self._files_frames_dev(lib().b200timg_jpeg_frames_dev, files, d_frames, d_status)
 
     def png_frames(self, files):
         """b200timg_png_frames: (list of [h, w, 4] uint8 canvases, int32 status per file) for a list of PNG files."""
-        files, bufs, sizes = _jpeg_args(files)
-        geo = [png_parse(f) for f in files] if files else []
-        total = sum(g["w"] * g["h"] * 4 for g in geo)
-        out = np.empty(max(1, total), np.uint8)
-        status = np.zeros(max(1, len(files)), np.int32)
-        self._chk(lib().b200timg_png_frames(self.h, len(files), bufs, sizes, out.ctypes.data, status.ctypes.data))
-        canv, o = [], 0
-        for g in geo:
-            canv.append(out[o:o + g["w"] * g["h"] * 4].reshape(g["h"], g["w"], 4))
-            o += g["w"] * g["h"] * 4
-        return canv, status[:len(files)]
+        return self._files_frames(lib().b200timg_png_frames, png_parse, files)
 
     def png_frames_dev(self, files, d_frames, d_status=None):
         """b200timg_png_frames_dev into a device tensor holding every canvas back to back (the src_offset layout of a
         mixed batch): returns d_status, an int32 device tensor with one entry per file, after the (asynchronous) call."""
-        import torch
-        files, bufs, sizes = _jpeg_args(files)
-        if d_status is None:
-            d_status = torch.empty(max(1, len(files)), dtype=torch.int32, device=d_frames.device)
-        self._chk(lib().b200timg_png_frames_dev(self.h, len(files), bufs, sizes, d_frames.data_ptr(), d_status.data_ptr()))
-        return d_status
+        return self._files_frames_dev(lib().b200timg_png_frames_dev, files, d_frames, d_status)
 
     @staticmethod
     def graphics_mixed_bound(b, g):

@@ -4,7 +4,7 @@
 #include <cmath>
 #include <cstdlib>
 
-#include "common.cuh"
+#include "decode.cuh"
 
 using namespace b200timg;
 
@@ -74,14 +74,8 @@ void b200timg_ctx_destroy(b200timg_ctx *ctx) {
     ctx->in_stage.release(); ctx->fb_scaled.release(); ctx->prev_stage.release();
     ctx->out_stage.release(); ctx->offsets.release(); ctx->cells.release(); ctx->rows.release();
     ctx->tables.release(); ctx->sixel_work.release(); ctx->misc.release(); ctx->scale_list.release(); ctx->scale_tmp.release(); ctx->tri_tables.release();
-    ctx->mixed_arena.release(); ctx->mixed_stage.release();
-    if (ctx->ev_mixed) cudaEventDestroy(ctx->ev_mixed);
-    ctx->gif_arena.release(); ctx->gif_scratch.release(); ctx->gif_stage.release();
-    if (ctx->ev_gif) cudaEventDestroy(ctx->ev_gif);
-    ctx->jpeg_arena.release(); ctx->jpeg_scratch.release(); ctx->jpeg_stage.release();
-    if (ctx->ev_jpeg) cudaEventDestroy(ctx->ev_jpeg);
-    ctx->png_arena.release(); ctx->png_scratch.release(); ctx->png_stage.release();
-    if (ctx->ev_png) cudaEventDestroy(ctx->ev_png);
+    ctx->mixed_up.release(); ctx->gif_up.release(); ctx->jpeg_up.release(); ctx->png_up.release();
+    ctx->gif_scratch.release(); ctx->jpeg_scratch.release(); ctx->png_scratch.release();
     ctx->pinned.release(); ctx->pinned_io.release();
     ctx->png_sums.release(); ctx->gfx_ids.release();
     ctx->dfl_raw.release(); ctx->dfl_scratch.release(); ctx->dfl_meta.release(); ctx->dfl_tokens.release(); ctx->dfl_png.release();
@@ -749,18 +743,6 @@ static int validate_mixed(b200timg_ctx *ctx, const b200timg_mixed_batch *b, bool
     return B200TIMG_OK;
 }
 
-// The plan's one upload.  The pinned staging is rewritten only after the previous mixed call's copy has run.
-static int mixed_upload(b200timg_ctx *ctx, const MixedPlan &mp) {
-    if (ctx->ev_mixed) B2_CUDA(ctx, cudaEventSynchronize(ctx->ev_mixed));
-    else B2_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_mixed, cudaEventDisableTiming));
-    B2_CUDA(ctx, ctx->mixed_stage.reserve(mp.arena.size()));
-    B2_CUDA(ctx, ctx->mixed_arena.reserve(mp.arena.size()));
-    memcpy(ctx->mixed_stage.p, mp.arena.data(), mp.arena.size());
-    B2_CUDA(ctx, cudaMemcpyAsync(ctx->mixed_arena.p, ctx->mixed_stage.p, mp.arena.size(), cudaMemcpyHostToDevice, ctx->stream));
-    B2_CUDA(ctx, cudaEventRecord(ctx->ev_mixed, ctx->stream));
-    return B200TIMG_OK;
-}
-
 int b200timg_scale_mixed_dev(b200timg_ctx *ctx, const b200timg_mixed_batch *b, const uint8_t *d_src, uint8_t *d_out) {
     B2_TRY(check_ctx(ctx));
     B2_TRY(validate_mixed(ctx, b, false));
@@ -769,9 +751,9 @@ int b200timg_scale_mixed_dev(b200timg_ctx *ctx, const b200timg_mixed_batch *b, c
         return ctx->fail(B200TIMG_EINVAL, "mixed batch: pixel buffers must be 4-byte aligned");
     MixedPlan mp;
     B2_TRY(plan_scale_mixed(ctx, b, mp));
-    B2_TRY(mixed_upload(ctx, mp));
+    B2_TRY(staged_upload(ctx, ctx->mixed_up, mp.arena));
     const ComposeSpec cs = make_compose_spec(b->has_bg, b->bg, b->pattern, b->pattern_w, b->pattern_h);
-    return launch_scale_mixed(ctx, mp, ctx->mixed_arena.as<char>(), d_src, d_out, b->n_frames, b->src_fmt == B200TIMG_FMT_RGB32, cs);
+    return launch_scale_mixed(ctx, mp, ctx->mixed_up.arena.as<char>(), d_src, d_out, b->n_frames, b->src_fmt == B200TIMG_FMT_RGB32, cs);
 }
 
 int b200timg_blocks_mixed_dev(b200timg_ctx *ctx, const b200timg_mixed_batch *b, const uint8_t *d_src,
@@ -785,11 +767,11 @@ int b200timg_blocks_mixed_dev(b200timg_ctx *ctx, const b200timg_mixed_batch *b, 
     B2_TRY(plan_blocks_mixed(ctx, b, mp));
     ctx->resident_fb = nullptr;
     B2_CUDA(ctx, ctx->fb_scaled.reserve((size_t)mp.out_px * 4));
-    B2_TRY(mixed_upload(ctx, mp));
+    B2_TRY(staged_upload(ctx, ctx->mixed_up, mp.arena));
     const ComposeSpec cs = make_compose_spec(b->has_bg, b->bg, b->pattern, b->pattern_w, b->pattern_h);
     uint8_t *d_fb = ctx->fb_scaled.as<uint8_t>();
-    B2_TRY(launch_scale_mixed(ctx, mp, ctx->mixed_arena.as<char>(), d_src, d_fb, b->n_frames, b->src_fmt == B200TIMG_FMT_RGB32, cs));
-    return launch_blocks_mixed(ctx, mp, ctx->mixed_arena.as<char>(), d_fb, b->n_frames, b->flags, d_out, out_cap, d_offsets);
+    B2_TRY(launch_scale_mixed(ctx, mp, ctx->mixed_up.arena.as<char>(), d_src, d_fb, b->n_frames, b->src_fmt == B200TIMG_FMT_RGB32, cs));
+    return launch_blocks_mixed(ctx, mp, ctx->mixed_up.arena.as<char>(), d_fb, b->n_frames, b->flags, d_out, out_cap, d_offsets);
 }
 
 // Host buffers: upload the sources, run the device variant into staging bounded by the sum of the frames' block bounds,
@@ -847,10 +829,10 @@ int b200timg_sixel_mixed_dev(b200timg_ctx *ctx, const b200timg_mixed_batch *b, c
     B2_TRY(plan_sixel_mixed(ctx, b, mp));
     ctx->resident_fb = nullptr;
     B2_CUDA(ctx, ctx->fb_scaled.reserve((size_t)mp.out_px * 4));
-    B2_TRY(mixed_upload(ctx, mp));
+    B2_TRY(staged_upload(ctx, ctx->mixed_up, mp.arena));
     const ComposeSpec cs = make_compose_spec(b->has_bg, b->bg, b->pattern, b->pattern_w, b->pattern_h);
     uint8_t *d_fb = ctx->fb_scaled.as<uint8_t>();
-    const char *d_arena = ctx->mixed_arena.as<char>();
+    const char *d_arena = ctx->mixed_up.arena.as<char>();
     B2_TRY(launch_scale_mixed(ctx, mp, d_arena, d_src, d_fb, b->n_frames, b->src_fmt == B200TIMG_FMT_RGB32, cs));
     B2_TRY(launch_pad_mixed(ctx, mp, d_arena, d_fb, b->n_frames, cs));
     return launch_sixel_mixed(ctx, mp, d_arena, d_fb, b->n_frames, d_out, out_cap, d_offsets);
@@ -909,10 +891,10 @@ int b200timg_graphics_mixed_dev(b200timg_ctx *ctx, const b200timg_mixed_batch *b
     B2_TRY(plan_graphics_mixed(ctx, b, gr, mp));
     ctx->resident_fb = nullptr;
     B2_CUDA(ctx, ctx->fb_scaled.reserve((size_t)mp.out_px * 4));
-    B2_TRY(mixed_upload(ctx, mp));
+    B2_TRY(staged_upload(ctx, ctx->mixed_up, mp.arena));
     const ComposeSpec cs = make_compose_spec(b->has_bg, b->bg, b->pattern, b->pattern_w, b->pattern_h);
     uint8_t *d_fb = ctx->fb_scaled.as<uint8_t>();
-    const char *d_arena = ctx->mixed_arena.as<char>();
+    const char *d_arena = ctx->mixed_up.arena.as<char>();
     B2_TRY(launch_scale_mixed(ctx, mp, d_arena, d_src, d_fb, b->n_frames, b->src_fmt == B200TIMG_FMT_RGB32, cs));
     return launch_graphics_mixed(ctx, mp, d_arena, d_fb, b->n_frames, gr, d_offsets, d_out, out_cap);
 }

@@ -47,6 +47,15 @@ struct HostBuf {   // pinned staging
     template <typename T> T *as() const { return reinterpret_cast<T *>(p); }
 };
 
+// One caller's host -> device upload (staged_upload, decode.cu): the pinned stage, the device arena it is copied to,
+// and the event that says the last copy out of the stage has run.
+struct Upload {
+    HostBuf stage;
+    DevBuf arena;
+    cudaEvent_t ev = nullptr;
+    void release() { stage.release(); arena.release(); if (ev) cudaEventDestroy(ev); ev = nullptr; }
+};
+
 }  // namespace b200timg
 
 namespace b200timg { struct ResamplePlan; void free_plan(ResamplePlan *); }
@@ -119,26 +128,15 @@ struct b200timg_ctx {
     cudaEvent_t ev_gather_ready = nullptr, ev_gather_done[4] = {nullptr, nullptr, nullptr, nullptr};
     uint64_t gather_seq = 0;
     b200timg::DevBuf gather_status;
-    // mixed batches (b200timg_mixed_batch): the call's tables and descriptors, uploaded in one copy from mixed_stage;
-    // the staging is rewritten only once ev_mixed says the previous call's copy has run
-    b200timg::DevBuf mixed_arena;
-    b200timg::HostBuf mixed_stage;
-    cudaEvent_t ev_mixed = nullptr;
-    // GIF decode (gif.cu): file + frame descriptors uploaded in one copy from gif_stage (rewritten once ev_gif says the
-    // previous call's copy has run), and the call's code streams, index planes and per-frame reach
-    b200timg::DevBuf gif_arena, gif_scratch;
-    b200timg::HostBuf gif_stage;
-    cudaEvent_t ev_gif = nullptr;
-    // JPEG decode (jpeg.cu): files + descriptors + Huffman tables uploaded in one copy from jpeg_stage (rewritten once
-    // ev_jpeg says the previous call's copy has run), and the call's streams, decoder states, coefficients and planes
-    b200timg::DevBuf jpeg_arena, jpeg_scratch;
-    b200timg::HostBuf jpeg_stage;
-    cudaEvent_t ev_jpeg = nullptr;
-    // PNG decode (png_decode.cu): files + descriptors uploaded in one copy from png_stage (rewritten once ev_png says
-    // the previous call's copy has run), and the call's zlib streams, raw planes, source indices and copy records
-    b200timg::DevBuf png_arena, png_scratch;
-    b200timg::HostBuf png_stage;
-    cudaEvent_t ev_png = nullptr;
+    // One upload per caller, so that a call waits only for the previous copy of its own kind:
+    //   mixed batches (b200timg_mixed_batch): the call's tables and descriptors;
+    //   GIF decode (gif.cu): file + frame descriptors;
+    //   JPEG decode (jpeg.cu): files + descriptors + Huffman tables;
+    //   PNG decode (png_decode.cu): files + descriptors.
+    b200timg::Upload mixed_up, gif_up, jpeg_up, png_up;
+    // the decoders' per-call scratch: GIF code streams, index planes and per-frame reach; JPEG streams, decoder
+    // states, coefficients and planes; PNG zlib streams, raw planes, source indices and copy records
+    b200timg::DevBuf gif_scratch, jpeg_scratch, png_scratch;
 
     int fail(int code, const char *fmt, ...) {
         va_list ap; va_start(ap, fmt);
@@ -189,6 +187,14 @@ struct b200timg_ctx {
     } while (0)
 
 namespace b200timg {
+
+// CTAs of `threads` threads for a grid-stride loop over `items`: one item per thread, at most 16 CTAs per SM, at least 1
+inline unsigned grid_for(b200timg_ctx *ctx, long long items, int threads = 256) {
+    long long b = (items + threads - 1) / threads;
+    const long long cap = (long long)ctx->sm_count * 16;
+    if (b > cap) b = cap;
+    return (unsigned)(b < 1 ? 1 : b);
+}
 
 // ---- strict IEEE-754 single precision, never contracted into FMA ------------------
 // The reference is compiled for baseline x86-64 (SSE2, no FMA): every * and + rounds
@@ -296,7 +302,7 @@ struct __align__(16) MixedBlocksFrame {
     int w, h, cols, rows, row_offset, indent;
 };
 // Everything the kernels of one mixed call read that the host computes, built once per call and uploaded in one copy
-// to ctx->mixed_arena: the scaler's tables and frame descriptors (plan_scale_mixed, resample.cu) and the block
+// to ctx->mixed_up.arena: the scaler's tables and frame descriptors (plan_scale_mixed, resample.cu) and the block
 // encoder's (plan_blocks_mixed, blocks.cu).
 struct MixedPlan {
     std::vector<char> arena;                       // host image of the upload

@@ -76,13 +76,6 @@ bbox_kernel(const uint32_t *__restrict__ in, int w, int h, int *__restrict__ rec
     }
 }
 
-static unsigned grid_for(b200timg_ctx *ctx, long long items) {
-    long long b = (items + 255) / 256;
-    const long long cap = (long long)ctx->sm_count * 16;
-    if (b > cap) b = cap;
-    return (unsigned)(b < 1 ? 1 : b);
-}
-
 int launch_exif(b200timg_ctx *ctx, const uint8_t *d_in, uint8_t *d_out, int w, int h, int mirror, int angle, int n_frames) {
     if (angle != 0 && angle != 180 && angle != 90 && angle != -90) return ctx->fail(B200TIMG_EINVAL, "exif: angle %d", angle);
     B2_KERNEL(ctx, "exif_kernel");

@@ -3,7 +3,8 @@
 // (third_party/stb/stb_image.h:6779-6951).
 //   host walk           the block structure, palette state, delays and every error visible without decoding a raster
 //                       (the walk ends each raster just after its terminator, as both of stb's raster exits do)
-//   gif_gather_kernel   drops the sub-block length bytes: every frame's payload as one contiguous code stream
+//   decode_gather_kernel (decode.cu) drops the sub-block length bytes: every frame's payload as one contiguous code
+//                       stream
 //   gif_lzw_kernel      one warp per frame: lane 0 walks the codes, the warp copies long strings; writes the frame's
 //                       index plane in stream order up to the rectangle's area, then only validates (:6694-6776)
 //   gif_compose_kernel  one thread per canvas pixel over the frames in order: dispose, overlay, first-frame background
@@ -11,7 +12,7 @@
 // A call launches these three kernels whatever its frame count.
 #include <algorithm>
 
-#include "common.cuh"
+#include "decode.cuh"
 
 namespace b200timg {
 
@@ -151,19 +152,6 @@ int walk_or_fail(b200timg_ctx *ctx, const uint8_t *gif, size_t size, Walk &wk) {
 }
 
 // ---- kernels ---------------------------------------------------------------------------------------------------
-// item g of the gathered payload: byte g - pay_start[s] of sub-block s (0 past the end of the file)
-__global__ void __launch_bounds__(256)
-gif_gather_kernel(const uint8_t *__restrict__ gif, unsigned long long size, const unsigned long long *__restrict__ sb_off,
-                  const unsigned long long *__restrict__ pay_start, int n_sb, uint8_t *__restrict__ payload) {
-    const unsigned long long total = n_sb > 0 ? pay_start[n_sb] : 0;
-    for (unsigned long long g = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; g < total;
-         g += (unsigned long long)gridDim.x * blockDim.x) {
-        const int s = mixed_owner(pay_start, n_sb, g);
-        const unsigned long long o = sb_off[s] + (g - pay_start[s]);
-        payload[g] = o < size ? gif[o] : 0;
-    }
-}
-
 // stbi__process_gif_raster with the dictionary as (start, len) into the frame's own index stream: an entry is always
 // the previous code's output plus the first byte of the current one, so no prefix chain is ever followed.
 constexpr int GIF_SHORT = 16;                      // strings up to this long are written by lane 0 alone
@@ -286,20 +274,13 @@ gif_compose_kernel(const GifFrame *__restrict__ desc, const uint32_t *__restrict
     }
 }
 
-unsigned grid_for(b200timg_ctx *ctx, long long items) {
-    long long b = (items + 255) / 256;
-    const long long cap = (long long)ctx->sm_count * 16;
-    if (b > cap) b = cap;
-    return (unsigned)(b < 1 ? 1 : b);
-}
-
-// Device scratch of one call (ctx->gif_arena + ctx->gif_scratch):
+// Device scratch of one call (ctx->gif_up.arena + ctx->gif_scratch):
 //   file + 80 n (descriptors) + 1024 n (palettes) + 4 sum(interlaced rh) + 16 S (S sub-blocks) + P (code streams)
 //   + sum(rw * rh) (index planes) + 8 n (reach), each part 16-byte aligned.
 int launch_gif(b200timg_ctx *ctx, const uint8_t *gif, size_t size, const Walk &wk, int n, uint8_t *d_frames, int32_t *d_valid) {
     std::vector<GifFrame> desc((size_t)n);
     std::vector<uint32_t> pal((size_t)n * 256), rank;
-    std::vector<unsigned long long> sb_off, pay_start(1, 0);
+    Runs runs;                                     // the sub-blocks of frames 0..n-1
     unsigned long long plane = 0;
     for (int f = 0; f < n; ++f) {
         const WalkFrame &w = wk.frames[(size_t)f];
@@ -308,9 +289,9 @@ int launch_gif(b200timg_ctx *ctx, const uint8_t *gif, size_t size, const Walk &w
         d.rx = w.rx; d.ry = w.ry; d.rw = w.rw; d.rh = w.rh; d.lzw_cs = w.lzw_cs; d.dispose2 = w.dispose2;
         d.interlaced = w.interlaced; d.bg_alt = w.bg_alt;
         d.plane = plane; plane += (unsigned long long)w.rw * w.rh;
-        d.code0 = pay_start.back();
-        for (size_t s = w.sb0; s < w.sb1; ++s) { sb_off.push_back(wk.sb_off[s]); pay_start.push_back(pay_start.back() + (unsigned)wk.sb_len[s]); }
-        d.code_len = pay_start.back() - d.code0;
+        d.code0 = runs.total();
+        for (size_t s = w.sb0; s < w.sb1; ++s) runs.add(wk.sb_off[s], (unsigned)wk.sb_len[s]);
+        d.code_len = runs.total() - d.code0;
         memcpy(&pal[(size_t)f * 256], w.pal, sizeof w.pal);
         d.rank0 = (unsigned)rank.size();
         if (w.interlaced) {                        // stb's pass loop (:6680-6689) at row granularity
@@ -324,41 +305,25 @@ int launch_gif(b200timg_ctx *ctx, const uint8_t *gif, size_t size, const Walk &w
             }
         }
     }
-    const int n_sb = (int)sb_off.size();
-    const unsigned long long paylen = pay_start.back();
+    const unsigned long long paylen = runs.total();
     std::vector<char> arena;
     const int32_t n32 = n;
     const size_t o_n = mixed_put(arena, &n32, sizeof n32);
     const size_t o_desc = mixed_put(arena, desc.data(), sizeof(GifFrame) * desc.size());
     const size_t o_pal = mixed_put(arena, pal.data(), sizeof(uint32_t) * pal.size());
     const size_t o_rank = mixed_put(arena, rank.data(), sizeof(uint32_t) * rank.size());
-    const size_t o_sb = mixed_put(arena, sb_off.data(), sizeof(unsigned long long) * sb_off.size());
-    const size_t o_ps = mixed_put(arena, pay_start.data(), sizeof(unsigned long long) * pay_start.size());
-    const size_t o_file = mixed_put(arena, nullptr, 0);
-    const size_t bytes = o_file + size;
-
-    // the previous call's upload has left the staging (the host waits for that copy only, not for its kernels)
-    if (ctx->ev_gif) B2_CUDA(ctx, cudaEventSynchronize(ctx->ev_gif));
-    else B2_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_gif, cudaEventDisableTiming));
-    B2_CUDA(ctx, ctx->gif_stage.reserve(bytes));
-    B2_CUDA(ctx, ctx->gif_arena.reserve(bytes));
-    memcpy(ctx->gif_stage.p, arena.data(), arena.size());
-    memcpy(ctx->gif_stage.as<char>() + o_file, gif, size);
-    B2_CUDA(ctx, cudaMemcpyAsync(ctx->gif_arena.p, ctx->gif_stage.p, bytes, cudaMemcpyHostToDevice, ctx->stream));
-    B2_CUDA(ctx, cudaEventRecord(ctx->ev_gif, ctx->stream));
+    runs.put(arena);
+    size_t o_file;
+    B2_TRY(staged_upload(ctx, ctx->gif_up, arena, 1, &gif, &size, &o_file));
     const size_t s_pay = 0, s_plane = (paylen + 15) / 16 * 16, s_reach = s_plane + (plane + 15) / 16 * 16;
     B2_CUDA(ctx, ctx->gif_scratch.reserve(s_reach + sizeof(unsigned long long) * (size_t)n));
-    const char *A = ctx->gif_arena.as<char>();
+    const char *A = ctx->gif_up.arena.as<char>();
     char *S = ctx->gif_scratch.as<char>();
     const GifFrame *d_desc = reinterpret_cast<const GifFrame *>(A + o_desc);
     unsigned long long *d_reach = reinterpret_cast<unsigned long long *>(S + s_reach);
     B2_CUDA(ctx, cudaMemcpyAsync(d_valid, A + o_n, sizeof(int32_t), cudaMemcpyDeviceToDevice, ctx->stream));
 
-    B2_KERNEL(ctx, "gif_gather_kernel");
-    gif_gather_kernel<<<grid_for(ctx, (long long)paylen), 256, 0, ctx->stream>>>(
-        reinterpret_cast<const uint8_t *>(A + o_file), size, reinterpret_cast<const unsigned long long *>(A + o_sb),
-        reinterpret_cast<const unsigned long long *>(A + o_ps), n_sb, reinterpret_cast<uint8_t *>(S + s_pay));
-    B2_LAUNCH_CHECK(ctx);
+    B2_TRY(launch_gather(ctx, runs, A, o_file, size, reinterpret_cast<uint8_t *>(S + s_pay)));
     B2_KERNEL(ctx, "gif_lzw_kernel");
     gif_lzw_kernel<<<n, 32, 0, ctx->stream>>>(d_desc, reinterpret_cast<const uint8_t *>(S + s_pay),
                                               reinterpret_cast<uint8_t *>(S + s_plane), d_reach, d_valid);
@@ -403,8 +368,7 @@ int b200timg_gif_frames_dev(b200timg_ctx *ctx, const uint8_t *gif, size_t size, 
     B2_CUDA(ctx, cudaSetDevice(ctx->device));
     Walk wk;
     B2_TRY(gif_frames_args(ctx, gif, size, n_frames, d_frames, d_valid, wk));
-    if (reinterpret_cast<uintptr_t>(d_frames) % 4 || reinterpret_cast<uintptr_t>(d_valid) % 4)
-        return ctx->fail(B200TIMG_EINVAL, "gif: d_frames and d_valid must be 4-byte aligned (whole RGBA pixels, int32)");
+    B2_TRY(check_dev_outputs(ctx, "gif", d_frames, d_valid, "d_valid"));
     return launch_gif(ctx, gif, size, wk, n_frames, d_frames, d_valid);
 }
 
@@ -413,17 +377,8 @@ int b200timg_gif_frames(b200timg_ctx *ctx, const uint8_t *gif, size_t size, int 
     B2_CUDA(ctx, cudaSetDevice(ctx->device));
     Walk wk;
     B2_TRY(gif_frames_args(ctx, gif, size, n_frames, frames, n_valid, wk));
-    const size_t bytes = (size_t)wk.w * wk.h * 4 * (size_t)n_frames;
-    B2_CUDA(ctx, ctx->in_stage.reserve(bytes));
-    B2_CUDA(ctx, ctx->misc.reserve(4096));
-    B2_CUDA(ctx, ctx->pinned.reserve(64));
-    int32_t *d_valid = reinterpret_cast<int32_t *>(ctx->misc.as<char>() + 2048);
-    B2_TRY(launch_gif(ctx, gif, size, wk, n_frames, ctx->in_stage.as<uint8_t>(), d_valid));
-    B2_CUDA(ctx, cudaMemcpyAsync(frames, ctx->in_stage.p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-    B2_CUDA(ctx, cudaMemcpyAsync(ctx->pinned.p, d_valid, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    B2_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    *n_valid = *ctx->pinned.as<int32_t>();
-    return B200TIMG_OK;
+    return decode_to_host(ctx, (size_t)wk.w * wk.h * 4 * (size_t)n_frames, 1, frames, n_valid,
+                          [&](uint8_t *d_frames, int32_t *d_valid) { return launch_gif(ctx, gif, size, wk, n_frames, d_frames, d_valid); });
 }
 
 }  // extern "C"

@@ -3,8 +3,8 @@
 // IDCT, colour conversion and hv_2 resampler (third_party/stb/stb_image.h:3822-3841).
 //   host walk              stbi__decode_jpeg_header / stbi__decode_jpeg_image's marker walk, Huffman and quantisation
 //                          tables as the scan sees them, and the scan's segments (restart intervals) as byte runs
-//   jpeg_destuff_kernel    the runs of every segment into one destuffed byte stream per segment (FF 00 and fill
-//                          bytes dropped)
+//   decode_gather_kernel   (decode.cu) the runs of every segment into one destuffed byte stream per segment (FF 00
+//                          and fill bytes dropped)
 //   jpeg_sync_kernel       self-synchronising Huffman decode (Weissenberger & Schmidt): each thread decodes its
 //                          64-byte subsequence from a guessed state until it passes the subsequence's end; a CTA
 //                          iterates until every start state equals its predecessor's exit
@@ -23,7 +23,7 @@
 #include <algorithm>
 #include <climits>
 
-#include "common.cuh"
+#include "decode.cuh"
 
 namespace b200timg {
 
@@ -540,17 +540,6 @@ __device__ __forceinline__ unsigned long long sub_end(const JpegSeg &g, unsigned
 }
 
 // ---- kernels -----------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-jpeg_destuff_kernel(const uint8_t *__restrict__ files, const unsigned long long *__restrict__ run_off,
-                    const unsigned long long *__restrict__ run_start, int n_runs, uint8_t *__restrict__ stream) {
-    const unsigned long long total = run_start[n_runs];
-    for (unsigned long long g = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; g < total;
-         g += (unsigned long long)gridDim.x * blockDim.x) {
-        const int r = mixed_owner(run_start, n_runs, g);
-        stream[g] = files[run_off[r] + (g - run_start[r])];
-    }
-}
-
 __global__ void __launch_bounds__(SYNC_T)
 jpeg_sync_kernel(const JpegFile *__restrict__ fd, const JpegSeg *__restrict__ sd, const unsigned *__restrict__ seg_sub,
                  int n_seg, const Huff *__restrict__ tabs, const uint8_t *__restrict__ stream, unsigned n_sub,
@@ -881,13 +870,6 @@ jpeg_color_kernel(const JpegFile *__restrict__ fd, const unsigned long long *__r
 namespace b200timg {
 namespace {
 
-unsigned grid_for(b200timg_ctx *ctx, long long items, int threads = 256) {
-    long long b = (items + threads - 1) / threads;
-    const long long cap = (long long)ctx->sm_count * 16;
-    if (b > cap) b = cap;
-    return (unsigned)(b < 1 ? 1 : b);
-}
-
 void fill_info(const Parse &P, b200timg_jpeg_info *info) {
     memset(info, 0, sizeof *info);
     info->w = P.w; info->h = P.h; info->n_comp = P.n;
@@ -898,21 +880,7 @@ void fill_info(const Parse &P, b200timg_jpeg_info *info) {
     snprintf(info->reason, sizeof info->reason, "%s", P.supported ? "" : P.why);
 }
 
-int parse_files(b200timg_ctx *ctx, int n, const uint8_t *const *files, const size_t *sizes, std::vector<Parse> &ps) {
-    if (n <= 0) return ctx->fail(B200TIMG_EINVAL, "jpeg: n_files %d <= 0", n);
-    if (!files || !sizes) return ctx->fail(B200TIMG_EINVAL, "jpeg: null files or sizes");
-    ps.resize((size_t)n);
-    for (int f = 0; f < n; ++f) {
-        if (!files[f] || sizes[f] == 0) return ctx->fail(B200TIMG_EINVAL, "jpeg: file %d has no data", f);
-        if (jpeg_walk(files[f], sizes[f], ps[(size_t)f]) != 0)
-            return ctx->fail(B200TIMG_EINVAL, "jpeg: file %d: stb's header walk fails", f);
-        if (!ps[(size_t)f].supported)
-            return ctx->fail(B200TIMG_EINVAL, "jpeg: file %d is not taken by the device: %s", f, ps[(size_t)f].why);
-    }
-    return B200TIMG_OK;
-}
-
-// Device scratch of one call (ctx->jpeg_arena + ctx->jpeg_scratch): the files + descriptors + deduplicated Huffman
+// Device scratch of one call (ctx->jpeg_up.arena + ctx->jpeg_scratch): the files + descriptors + deduplicated Huffman
 // tables (2.4 KB each) + 16 bytes per byte run; destuffed streams, 20 bytes per 64-byte subsequence, 132 bytes per
 // 8x8 block (coefficients and DC difference), the component planes (sum of w2 * h2), 8 bytes per file.
 int launch_jpeg(b200timg_ctx *ctx, int n, const uint8_t *const *files, const size_t *sizes, const std::vector<Parse> &ps,
@@ -920,7 +888,8 @@ int launch_jpeg(b200timg_ctx *ctx, int n, const uint8_t *const *files, const siz
     std::vector<JpegFile> fdesc((size_t)n);
     std::vector<JpegSeg> sdesc;
     std::vector<Huff> tabs;
-    std::vector<unsigned long long> run_off, run_start(1, 0), file_unit0(1, 0), file_px0(1, 0);
+    Runs runs;
+    std::vector<unsigned long long> file_unit0(1, 0), file_px0(1, 0);
     std::vector<unsigned> seg_sub(1, 0);
     unsigned long long plane = 0, file_off = 0, stream = 0;
     unsigned nsub = 0;
@@ -981,14 +950,14 @@ int launch_jpeg(b200timg_ctx *ctx, int n, const uint8_t *const *files, const siz
             g.nsub = (unsigned)std::max<unsigned long long>(1, (hs.L + SUB_BYTES - 1) / SUB_BYTES);
             nsub += g.nsub;
             seg_sub.push_back(nsub);
-            for (const Run &r : hs.runs) { run_off.push_back(file_off + r.off); run_start.push_back(run_start.back() + r.len); }
+            for (const Run &r : hs.runs) runs.add(file_off + r.off, r.len);
             stream += hs.L;
             sdesc.push_back(g);
         }
         file_off += sizes[fi];
     }
     seg_sub.pop_back();
-    const int n_seg = (int)sdesc.size(), n_runs = (int)run_off.size();
+    const int n_seg = (int)sdesc.size();
     const unsigned long long units = file_unit0.back();
     if (units > (1ull << 31)) return ctx->fail(B200TIMG_EINVAL, "jpeg: %llu blocks in one call (at most 2^31)", units);
 
@@ -997,31 +966,17 @@ int launch_jpeg(b200timg_ctx *ctx, int n, const uint8_t *const *files, const siz
     const size_t o_sd = mixed_put(arena, sdesc.data(), sizeof(JpegSeg) * sdesc.size());
     const size_t o_tab = mixed_put(arena, tabs.data(), sizeof(Huff) * tabs.size());
     const size_t o_ss = mixed_put(arena, seg_sub.data(), sizeof(unsigned) * seg_sub.size());
-    const size_t o_ro = mixed_put(arena, run_off.data(), sizeof(unsigned long long) * run_off.size());
-    const size_t o_rs = mixed_put(arena, run_start.data(), sizeof(unsigned long long) * run_start.size());
+    runs.put(arena);
     const size_t o_fu = mixed_put(arena, file_unit0.data(), sizeof(unsigned long long) * file_unit0.size());
     const size_t o_fp = mixed_put(arena, file_px0.data(), sizeof(unsigned long long) * file_px0.size());
-    const size_t o_file = mixed_put(arena, nullptr, 0);
-    const size_t bytes = o_file + file_off;
-
-    // the previous call's upload has left the staging (the host waits for that copy only, not for its kernels)
-    if (ctx->ev_jpeg) B2_CUDA(ctx, cudaEventSynchronize(ctx->ev_jpeg));
-    else B2_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_jpeg, cudaEventDisableTiming));
-    B2_CUDA(ctx, ctx->jpeg_stage.reserve(bytes));
-    B2_CUDA(ctx, ctx->jpeg_arena.reserve(bytes));
-    memcpy(ctx->jpeg_stage.p, arena.data(), arena.size());
-    {
-        char *dst = ctx->jpeg_stage.as<char>() + o_file;
-        for (int fi = 0; fi < n; ++fi) { memcpy(dst, files[fi], sizes[fi]); dst += sizes[fi]; }
-    }
-    B2_CUDA(ctx, cudaMemcpyAsync(ctx->jpeg_arena.p, ctx->jpeg_stage.p, bytes, cudaMemcpyHostToDevice, ctx->stream));
-    B2_CUDA(ctx, cudaEventRecord(ctx->ev_jpeg, ctx->stream));
+    size_t o_file;
+    B2_TRY(staged_upload(ctx, ctx->jpeg_up, arena, n, files, sizes, &o_file));
     auto al = [](unsigned long long v) { return (v + 255) / 256 * 256; };
     const size_t s_stream = 0, s_st = al(stream), s_ex = s_st + al(8ull * nsub), s_cnt = s_ex + al(8ull * nsub),
                  s_us = s_cnt + al(4ull * nsub), s_coef = s_us + al(4ull * nsub), s_dc = s_coef + al(128ull * units),
                  s_plane = s_dc + al(4ull * units), s_key = s_plane + al(plane), s_end = s_key + al(8ull * n);
     B2_CUDA(ctx, ctx->jpeg_scratch.reserve(s_end));
-    const char *A = ctx->jpeg_arena.as<char>();
+    const char *A = ctx->jpeg_up.arena.as<char>();
     char *S = ctx->jpeg_scratch.as<char>();
     const JpegFile *d_fd = reinterpret_cast<const JpegFile *>(A + o_fd);
     const JpegSeg *d_sd = reinterpret_cast<const JpegSeg *>(A + o_sd);
@@ -1038,11 +993,7 @@ int launch_jpeg(b200timg_ctx *ctx, int n, const uint8_t *const *files, const siz
     unsigned long long *d_key = reinterpret_cast<unsigned long long *>(S + s_key);
     B2_CUDA(ctx, cudaMemsetAsync(d_key, 0xff, 8ull * n, ctx->stream));
 
-    B2_KERNEL(ctx, "jpeg_destuff_kernel");
-    jpeg_destuff_kernel<<<grid_for(ctx, (long long)stream), 256, 0, ctx->stream>>>(
-        reinterpret_cast<const uint8_t *>(A + o_file), reinterpret_cast<const unsigned long long *>(A + o_ro),
-        reinterpret_cast<const unsigned long long *>(A + o_rs), n_runs, reinterpret_cast<uint8_t *>(S + s_stream));
-    B2_LAUNCH_CHECK(ctx);
+    B2_TRY(launch_gather(ctx, runs, A, o_file, file_off, reinterpret_cast<uint8_t *>(S + s_stream)));
     B2_KERNEL(ctx, "jpeg_sync_kernel");
     jpeg_sync_kernel<<<(nsub + SYNC_T - 2) / (SYNC_T - 1), SYNC_T, 0, ctx->stream>>>(d_fd, d_sd, d_ss, n_seg, d_tab, d_stream,
                                                                                    nsub, d_st, d_ex, d_cnt);
@@ -1088,11 +1039,9 @@ int b200timg_jpeg_frames_dev(b200timg_ctx *ctx, int n_files, const uint8_t *cons
                              uint8_t *d_frames, int32_t *d_status) {
     if (!ctx) return B200TIMG_EINVAL;
     B2_CUDA(ctx, cudaSetDevice(ctx->device));
-    if (!d_frames || !d_status) return ctx->fail(B200TIMG_EINVAL, "jpeg: null output");
-    if (reinterpret_cast<uintptr_t>(d_frames) % 4 || reinterpret_cast<uintptr_t>(d_status) % 4)
-        return ctx->fail(B200TIMG_EINVAL, "jpeg: d_frames and d_status must be 4-byte aligned (whole RGBA pixels, int32)");
+    B2_TRY(check_dev_outputs(ctx, "jpeg", d_frames, d_status, "d_status"));
     std::vector<Parse> ps;
-    B2_TRY(parse_files(ctx, n_files, files, sizes, ps));
+    B2_TRY(parse_files(ctx, "jpeg", "header walk", jpeg_walk, n_files, files, sizes, ps));
     return launch_jpeg(ctx, n_files, files, sizes, ps, d_frames, d_status);
 }
 
@@ -1102,18 +1051,12 @@ int b200timg_jpeg_frames(b200timg_ctx *ctx, int n_files, const uint8_t *const *f
     B2_CUDA(ctx, cudaSetDevice(ctx->device));
     if (!frames || !status) return ctx->fail(B200TIMG_EINVAL, "jpeg: null output");
     std::vector<Parse> ps;
-    B2_TRY(parse_files(ctx, n_files, files, sizes, ps));
+    B2_TRY(parse_files(ctx, "jpeg", "header walk", jpeg_walk, n_files, files, sizes, ps));
     size_t bytes = 0;
     for (const Parse &P : ps) bytes += (size_t)P.w * P.h * 4;
-    B2_CUDA(ctx, ctx->in_stage.reserve(bytes + 4 * (size_t)n_files + 16));
-    B2_CUDA(ctx, ctx->pinned.reserve(4 * (size_t)n_files + 64));
-    int32_t *d_status = reinterpret_cast<int32_t *>(ctx->in_stage.as<char>() + (bytes + 15) / 16 * 16);
-    B2_TRY(launch_jpeg(ctx, n_files, files, sizes, ps, ctx->in_stage.as<uint8_t>(), d_status));
-    B2_CUDA(ctx, cudaMemcpyAsync(frames, ctx->in_stage.p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-    B2_CUDA(ctx, cudaMemcpyAsync(ctx->pinned.p, d_status, 4 * (size_t)n_files, cudaMemcpyDeviceToHost, ctx->stream));
-    B2_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    memcpy(status, ctx->pinned.p, 4 * (size_t)n_files);
-    return B200TIMG_OK;
+    return decode_to_host(ctx, bytes, n_files, frames, status, [&](uint8_t *d_frames, int32_t *d_status) {
+        return launch_jpeg(ctx, n_files, files, sizes, ps, d_frames, d_status);
+    });
 }
 
 }  // extern "C"

@@ -3,7 +3,7 @@
 // png.cu is the encoder; this file only decodes.
 //   host walk              stbi__parse_png_file's chunk walk (third_party/stb/stb_image.h:5079-5262) without
 //                          inflating: IHDR, PLTE / tRNS as stb's palette array sees them, the IDAT payloads as runs
-//   png_gather_kernel      the IDAT payloads of every file into one zlib stream per file
+//   decode_gather_kernel   (decode.cu) the IDAT payloads of every file into one zlib stream per file
 //   png_inflate_kernel     one CTA per file: stb's zlib reader (:4125-4509), restated bit for bit.  Thread 0 reads the
 //                          block headers; the symbols of a Huffman block are decoded by every thread of the CTA
 //                          (self-synchronising subsequences, as jpeg_sync_kernel), thread 0 alone only in the last
@@ -22,7 +22,7 @@
 #include <algorithm>
 #include <climits>
 
-#include "common.cuh"
+#include "decode.cuh"
 
 namespace b200timg {
 
@@ -893,29 +893,11 @@ png_color_kernel(const PngFile *__restrict__ fd, const unsigned long long *__res
     }
 }
 
-__global__ void __launch_bounds__(256)
-png_gather_kernel(const uint8_t *__restrict__ files, const unsigned long long *__restrict__ run_off,
-                  const unsigned long long *__restrict__ run_start, int n_runs, uint8_t *__restrict__ stream) {
-    const unsigned long long total = run_start[n_runs];
-    for (unsigned long long g = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; g < total;
-         g += (unsigned long long)gridDim.x * blockDim.x) {
-        const int r = mixed_owner(run_start, n_runs, g);
-        stream[g] = files[run_off[r] + (g - run_start[r])];
-    }
-}
-
 }  // namespace
 }  // namespace b200timg
 
 namespace b200timg {
 namespace {
-
-unsigned grid_for(b200timg_ctx *ctx, long long items, int threads = 256) {
-    long long b = (items + threads - 1) / threads;
-    const long long cap = (long long)ctx->sm_count * 16;
-    if (b > cap) b = cap;
-    return (unsigned)(b < 1 ? 1 : b);
-}
 
 void fill_info(const Parse &P, b200timg_png_info *info) {
     memset(info, 0, sizeof *info);
@@ -930,28 +912,15 @@ void fill_info(const Parse &P, b200timg_png_info *info) {
     snprintf(info->reason, sizeof info->reason, "%s", P.supported ? "" : P.why);
 }
 
-int parse_files(b200timg_ctx *ctx, int n, const uint8_t *const *files, const size_t *sizes, std::vector<Parse> &ps) {
-    if (n <= 0) return ctx->fail(B200TIMG_EINVAL, "png: n_files %d <= 0", n);
-    if (!files || !sizes) return ctx->fail(B200TIMG_EINVAL, "png: null files or sizes");
-    ps.resize((size_t)n);
-    for (int f = 0; f < n; ++f) {
-        if (!files[f] || sizes[f] == 0) return ctx->fail(B200TIMG_EINVAL, "png: file %d has no data", f);
-        if (png_walk(files[f], sizes[f], ps[(size_t)f]) != 0)
-            return ctx->fail(B200TIMG_EINVAL, "png: file %d: stb's chunk walk fails", f);
-        if (!ps[(size_t)f].supported)
-            return ctx->fail(B200TIMG_EINVAL, "png: file %d is not taken by the device: %s", f, ps[(size_t)f].why);
-    }
-    return B200TIMG_OK;
-}
-
-// Device scratch of one call (ctx->png_arena + ctx->png_scratch): the files + 1.2 KB per file + 32 bytes per image +
+// Device scratch of one call (ctx->png_up.arena + ctx->png_scratch): the files + 1.2 KB per file + 32 bytes per image +
 // 16 bytes per IDAT; the zlib streams, 6 bytes per raw byte the images read (literal plane, source index, filtered
 // plane), 8 bytes per copy record (at most need / 3 + 1 per file), 8 bytes per file.
 int launch_png(b200timg_ctx *ctx, int n, const uint8_t *const *files, const size_t *sizes, const std::vector<Parse> &ps,
                uint8_t *d_frames, int32_t *d_status) {
     std::vector<PngFile> fdesc((size_t)n);
     std::vector<PngImage> imgs;
-    std::vector<unsigned long long> run_off, run_start(1, 0), file_raw0(1, 0), file_px0(1, 0);
+    Runs runs;
+    std::vector<unsigned long long> file_raw0(1, 0), file_px0(1, 0);
     unsigned long long file_off = 0, stream = 0, recs = 0;
     for (int fi = 0; fi < n; ++fi) {
         const Parse &P = ps[(size_t)fi];
@@ -960,7 +929,7 @@ int launch_png(b200timg_ctx *ctx, int n, const uint8_t *const *files, const size
         F.px0 = file_px0.back();
         file_px0.push_back(F.px0 + (unsigned long long)P.w * P.h);
         F.stream0 = stream; F.L = P.idat_bytes;
-        for (const Run &r : P.idat) { run_off.push_back(file_off + r.off); run_start.push_back(run_start.back() + r.len); }
+        for (const Run &r : P.idat) runs.add(file_off + r.off, r.len);
         stream += P.idat_bytes;
         F.raw0 = file_raw0.back(); F.need = P.need;
         file_raw0.push_back(F.raw0 + P.need);
@@ -996,36 +965,22 @@ int launch_png(b200timg_ctx *ctx, int n, const uint8_t *const *files, const size
     const unsigned long long raw_total = file_raw0.back();
     if (raw_total >= (1ull << 32))
         return ctx->fail(B200TIMG_EINVAL, "png: %llu raw bytes in one call (less than 2^32)", raw_total);
-    const int n_runs = (int)run_off.size(), n_img = (int)imgs.size();
+    const int n_img = (int)imgs.size();
 
     std::vector<char> arena;
     const size_t o_fd = mixed_put(arena, fdesc.data(), sizeof(PngFile) * fdesc.size());
     const size_t o_im = mixed_put(arena, imgs.data(), sizeof(PngImage) * imgs.size());
-    const size_t o_ro = mixed_put(arena, run_off.data(), sizeof(unsigned long long) * run_off.size());
-    const size_t o_rs = mixed_put(arena, run_start.data(), sizeof(unsigned long long) * run_start.size());
+    runs.put(arena);
     const size_t o_fr = mixed_put(arena, file_raw0.data(), sizeof(unsigned long long) * file_raw0.size());
     const size_t o_fp = mixed_put(arena, file_px0.data(), sizeof(unsigned long long) * file_px0.size());
-    const size_t o_file = mixed_put(arena, nullptr, 0);
-    const size_t bytes = o_file + file_off;
-
-    // the previous call's upload has left the staging (the host waits for that copy only, not for its kernels)
-    if (ctx->ev_png) B2_CUDA(ctx, cudaEventSynchronize(ctx->ev_png));
-    else B2_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_png, cudaEventDisableTiming));
-    B2_CUDA(ctx, ctx->png_stage.reserve(bytes));
-    B2_CUDA(ctx, ctx->png_arena.reserve(bytes));
-    memcpy(ctx->png_stage.p, arena.data(), arena.size());
-    {
-        char *dst = ctx->png_stage.as<char>() + o_file;
-        for (int fi = 0; fi < n; ++fi) { memcpy(dst, files[fi], sizes[fi]); dst += sizes[fi]; }
-    }
-    B2_CUDA(ctx, cudaMemcpyAsync(ctx->png_arena.p, ctx->png_stage.p, bytes, cudaMemcpyHostToDevice, ctx->stream));
-    B2_CUDA(ctx, cudaEventRecord(ctx->ev_png, ctx->stream));
+    size_t o_file;
+    B2_TRY(staged_upload(ctx, ctx->png_up, arena, n, files, sizes, &o_file));
     auto al = [](unsigned long long v) { return (v + 255) / 256 * 256; };
     const size_t s_stream = 0, s_raw = al(stream), s_src = s_raw + al(raw_total), s_flt = s_src + al(4 * raw_total),
                  s_rec = s_flt + al(raw_total), s_nrec = s_rec + al(8 * recs), s_key = s_nrec + al(4ull * n),
                  s_ch = s_key + al(4ull * n), s_end = s_ch + al(4ull * JUMP_ROUNDS);
     B2_CUDA(ctx, ctx->png_scratch.reserve(s_end));
-    const char *A = ctx->png_arena.as<char>();
+    const char *A = ctx->png_up.arena.as<char>();
     char *S = ctx->png_scratch.as<char>();
     const PngFile *d_fd = reinterpret_cast<const PngFile *>(A + o_fd);
     const unsigned long long *d_fr = reinterpret_cast<const unsigned long long *>(A + o_fr);
@@ -1039,11 +994,7 @@ int launch_png(b200timg_ctx *ctx, int n, const uint8_t *const *files, const size
     unsigned *d_ch = reinterpret_cast<unsigned *>(S + s_ch);
     B2_CUDA(ctx, cudaMemsetAsync(d_ch, 0, 4ull * JUMP_ROUNDS, ctx->stream));
 
-    B2_KERNEL(ctx, "png_gather_kernel");
-    png_gather_kernel<<<grid_for(ctx, (long long)stream), 256, 0, ctx->stream>>>(
-        reinterpret_cast<const uint8_t *>(A + o_file), reinterpret_cast<const unsigned long long *>(A + o_ro),
-        reinterpret_cast<const unsigned long long *>(A + o_rs), n_runs, d_stream);
-    B2_LAUNCH_CHECK(ctx);
+    B2_TRY(launch_gather(ctx, runs, A, o_file, file_off, d_stream));
     B2_KERNEL(ctx, "png_inflate_kernel");
     png_inflate_kernel<<<n, INF_T, 0, ctx->stream>>>(d_fd, d_stream, d_raw, d_rec, d_nrec, d_key);
     B2_LAUNCH_CHECK(ctx);
@@ -1088,11 +1039,9 @@ int b200timg_png_frames_dev(b200timg_ctx *ctx, int n_files, const uint8_t *const
                             uint8_t *d_frames, int32_t *d_status) {
     if (!ctx) return B200TIMG_EINVAL;
     B2_CUDA(ctx, cudaSetDevice(ctx->device));
-    if (!d_frames || !d_status) return ctx->fail(B200TIMG_EINVAL, "png: null output");
-    if (reinterpret_cast<uintptr_t>(d_frames) % 4 || reinterpret_cast<uintptr_t>(d_status) % 4)
-        return ctx->fail(B200TIMG_EINVAL, "png: d_frames and d_status must be 4-byte aligned (whole RGBA pixels, int32)");
+    B2_TRY(check_dev_outputs(ctx, "png", d_frames, d_status, "d_status"));
     std::vector<Parse> ps;
-    B2_TRY(parse_files(ctx, n_files, files, sizes, ps));
+    B2_TRY(parse_files(ctx, "png", "chunk walk", png_walk, n_files, files, sizes, ps));
     return launch_png(ctx, n_files, files, sizes, ps, d_frames, d_status);
 }
 
@@ -1102,18 +1051,12 @@ int b200timg_png_frames(b200timg_ctx *ctx, int n_files, const uint8_t *const *fi
     B2_CUDA(ctx, cudaSetDevice(ctx->device));
     if (!frames || !status) return ctx->fail(B200TIMG_EINVAL, "png: null output");
     std::vector<Parse> ps;
-    B2_TRY(parse_files(ctx, n_files, files, sizes, ps));
+    B2_TRY(parse_files(ctx, "png", "chunk walk", png_walk, n_files, files, sizes, ps));
     size_t bytes = 0;
     for (const Parse &P : ps) bytes += (size_t)P.w * P.h * 4;
-    B2_CUDA(ctx, ctx->in_stage.reserve(bytes + 4 * (size_t)n_files + 16));
-    B2_CUDA(ctx, ctx->pinned.reserve(4 * (size_t)n_files + 64));
-    int32_t *d_status = reinterpret_cast<int32_t *>(ctx->in_stage.as<char>() + (bytes + 15) / 16 * 16);
-    B2_TRY(launch_png(ctx, n_files, files, sizes, ps, ctx->in_stage.as<uint8_t>(), d_status));
-    B2_CUDA(ctx, cudaMemcpyAsync(frames, ctx->in_stage.p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-    B2_CUDA(ctx, cudaMemcpyAsync(ctx->pinned.p, d_status, 4 * (size_t)n_files, cudaMemcpyDeviceToHost, ctx->stream));
-    B2_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    memcpy(status, ctx->pinned.p, 4 * (size_t)n_files);
-    return B200TIMG_OK;
+    return decode_to_host(ctx, bytes, n_files, frames, status, [&](uint8_t *d_frames, int32_t *d_status) {
+        return launch_png(ctx, n_files, files, sizes, ps, d_frames, d_status);
+    });
 }
 
 }  // extern "C"

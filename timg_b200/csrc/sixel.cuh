@@ -43,7 +43,7 @@ struct __align__(16) MixedSixelFrame {
     int band0, prog0;                  // first flat band (band_bytes / band_off) and first progress flag
     int cols_per_warp, bands_per_cta;  // emit5's column split; the dither's bands per CTA
 };
-// What the mixed kernels read besides SixelWork: the descriptors and the flat item lists (all in ctx->mixed_arena).
+// What the mixed kernels read besides SixelWork: the descriptors and the flat item lists (all in ctx->mixed_up.arena).
 struct MixedSixelParams {
     const MixedSixelFrame *desc;
     const unsigned *band_start;        // [n + 1] first flat band of each frame (emit, compaction)
