@@ -136,8 +136,13 @@ def samples(w, h, color, depth, seed=0):
 
 # ---- deflate bit writer ---------------------------------------------------------------------------------------------
 class BitWriter:
+    """Bits LSB first.  marks: the bit at which each symbol op of fixed() / dynamic() starts (the end-of-block
+    included); blocks: (header bit, first symbol or stored-data bit) of each block -- so a test can place an event to
+    the bit (a 7- or 9-bit fixed literal moves every later mark by one)."""
     def __init__(self):
         self.bits = []
+        self.marks = []
+        self.blocks = []
 
     def put(self, v, n):                           # n bits of v, LSB first (header fields, extra bits)
         self.bits += [(v >> i) & 1 for i in range(n)]
@@ -150,8 +155,7 @@ class BitWriter:
             self.bits.append(0)
 
     def bytes(self):
-        b = self.bits + [0] * (-len(self.bits) % 8)
-        return bytes(sum(b[i + k] << k for k in range(8)) for i in range(0, len(b), 8))
+        return np.packbits(np.asarray(self.bits, np.uint8), bitorder="little").tobytes()
 
 
 def canonical(lengths):
@@ -185,6 +189,7 @@ DIST_EXTRA = [0, 0, 0, 0, 1, 1, 2, 2, 3, 3, 4, 4, 5, 5, 6, 6, 7, 7, 8, 8, 9, 9, 
 def _symbols(bw, ops, lit, dist):
     """ops: ints (literal / symbol), ('copy', length, distance) or ('sym', lit_symbol) / ('dsym', lit, dist_sym)."""
     for op in ops:
+        bw.marks.append(len(bw.bits))
         if isinstance(op, int):
             bw.code(*lit[op])
         elif op[0] == "copy":
@@ -202,26 +207,32 @@ def _symbols(bw, ops, lit, dist):
             bw.put(op[1], op[2])
 
 
-def stored(bw, data, final, nlen=None):
+def stored(bw, data, final, nlen=None, n=None):
+    """A stored block; n: the LEN field if not len(data)."""
+    start = len(bw.bits)
     bw.put(final, 1)
     bw.put(0, 2)
     bw.align()
-    n = len(data)
+    n = len(data) if n is None else n
     bw.put(n, 16)
     bw.put((n ^ 0xffff) if nlen is None else nlen, 16)
+    bw.blocks.append((start, len(bw.bits)))
     for b in data:
         bw.put(b, 8)
 
 
 def fixed(bw, ops, final):
+    start = len(bw.bits)
     bw.put(final, 1)
     bw.put(1, 2)
+    bw.blocks.append((start, len(bw.bits)))
     _symbols(bw, list(ops) + [256], canonical(FIXED_LIT), canonical(FIXED_DIST))
 
 
 def dynamic(bw, ops, final, lit_lengths, dist_lengths, clen_seq=None, end=True):
     """A dynamic block whose code lengths are sent one literal code-length symbol each (a 5-bit code for all 19
     code-length symbols), unless clen_seq gives the raw code-length symbol sequence as (symbol, extra value) pairs."""
+    start = len(bw.bits)
     bw.put(final, 1)
     bw.put(2, 2)
     hlit, hdist = len(lit_lengths), len(dist_lengths)
@@ -240,6 +251,7 @@ def dynamic(bw, ops, final, lit_lengths, dist_lengths, clen_seq=None, end=True):
             bw.put(extra, 3)
         elif sym == 18:
             bw.put(extra, 7)
+    bw.blocks.append((start, len(bw.bits)))
     _symbols(bw, list(ops) + ([256] if end else []), canonical(lit_lengths), canonical(dist_lengths))
 
 
