@@ -519,6 +519,39 @@ int b200timg_png_frames_dev(b200timg_ctx *ctx, int n_files, const uint8_t *const
 int b200timg_png_frames(b200timg_ctx *ctx, int n_files, const uint8_t *const *files, const size_t *sizes,
                         uint8_t *frames, int32_t *status);
 
+/* ======================= QOI files: the QOI source's decode ===================
+ * timg tries its QOI source before STB for every file (ImageSource::Create, src/image-source.cc:170-211).  File f's
+ * canvas is the w*h*4 RGBA buffer qoi_read(filename, &desc, 4) returns for it (third_party/qoi/qoi.h:488-646), which
+ * is what src/qoi-image-source.cc:42-77 scales, quirks included: the ops are the bytes [14, size - 8) whatever the last
+ * 8 bytes hold (an op starting there may read into them), every pixel after the ops run out repeats the last value, ops
+ * past the last pixel are ignored, an INDEX of a slot never written gives {0,0,0,0}, and the header's channel count
+ * does not reach the ops: a 3-channel file can carry alpha.
+ *
+ * Host only: qoi_decode's header checks.  B200TIMG_EINVAL exactly where qoi_decode returns NULL (fewer than 22 bytes,
+ * a bad magic, w or h 0, channels not 3 or 4, colorspace > 1, h >= 400000000 / w), so the reference's QOI source fails
+ * and an adapter falls through to the STB source.  supported = 0 (reason says why) for files of 2^31 bytes or more,
+ * whose size qoi_read holds in an int. */
+typedef struct {
+    int w, h, channels, colorspace;
+    int supported;
+    char reason[96];
+} b200timg_qoi_info;
+int b200timg_qoi_parse(const uint8_t *qoi, size_t size, b200timg_qoi_info *info);
+/* Canvases of n_files files back to back: file f at d_frames + sum_{g<f} w_g*h_g*4, the src_offset layout of a
+ * b200timg_mixed_batch with B200TIMG_FMT_RGBA.  files: HOST bytes, uploaded in one copy through context-owned pinned
+ * staging (the call waits on the host for the previous call's upload before it rewrites the staging, never for its
+ * own work).  d_status[f] (device): 1 the canvas is the reference's and timg composes it like the rest of the page (a
+ * 4-channel file, or a 3-channel file whose alpha is all 255); 2 the canvas is the reference's but timg does not
+ * compose it (a 3-channel header with some alpha below 255).  A file that parses always decodes.  B200TIMG_EINVAL
+ * before any launch, naming the file: a file b200timg_qoi_parse rejects or reports unsupported, n_files <= 0,
+ * d_frames or d_status not 4-byte aligned, 2^36 op bytes or more in one call.  A call launches 15 kernels whatever
+ * n_files is and whatever the files hold. */
+int b200timg_qoi_frames_dev(b200timg_ctx *ctx, int n_files, const uint8_t *const *files, const size_t *sizes,
+                            uint8_t *d_frames, int32_t *d_status);
+/* Host form: frames gets the canvases back to back, status[f] as above. */
+int b200timg_qoi_frames(b200timg_ctx *ctx, int n_files, const uint8_t *const *files, const size_t *sizes,
+                        uint8_t *frames, int32_t *status);
+
 /* ======================= Kitty / iTerm2 canvases: PNG + base64 (SURVEY 8f rank 2) ===================
  * png::Encode (src/timg-png.cc:90-152): signature, IHDR, one IDAT holding the zlib stream of the scanlines (each
  * row filtered with "Sub"), IEND.  rgb24 != 0: colour type 2 (png::ColorEncoding::kRGB_24), else RGBA.  The

@@ -168,6 +168,9 @@ ABI = {
     "b200timg_png_parse": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200timg_png_frames_dev": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200timg_png_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200timg_qoi_parse": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200timg_qoi_frames_dev": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200timg_qoi_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 _lib = None
@@ -323,6 +326,23 @@ def png_parse(data):
     return dict(w=info.w, h=info.h, bit_depth=info.bit_depth, color_type=info.color_type, interlace=info.interlace,
                 palette_len=info.palette_len, trns=info.trns, cgbi=bool(info.cgbi), apng=bool(info.apng),
                 idat_bytes=info.idat_bytes, supported=bool(info.supported), reason=info.reason.decode())
+
+
+class QoiInfo(C.Structure):
+    _fields_ = [("w", C.c_int), ("h", C.c_int), ("channels", C.c_int), ("colorspace", C.c_int), ("supported", C.c_int),
+                ("reason", C.c_char * 96)]
+
+
+def qoi_parse(data):
+    """b200timg_qoi_parse (host only): a dict of w, h, channels, colorspace, supported and reason.  Raises
+    B200Error(EINVAL) where qoi_decode returns NULL (so the reference's QOI source fails and timg tries STB)."""
+    data = bytes(data)
+    info = QoiInfo()
+    rc = lib().b200timg_qoi_parse(data, len(data), C.byref(info))
+    if rc != OK:
+        raise B200Error(rc, "qoi_parse: qoi_decode rejects the header")
+    return dict(w=info.w, h=info.h, channels=info.channels, colorspace=info.colorspace,
+                supported=bool(info.supported), reason=info.reason.decode())
 
 
 def _file_args(files):
@@ -690,7 +710,7 @@ class Context:
         return d_valid
 
     def _files_frames(self, fn, parse, files):
-        """The host form of a multi-file decode (jpeg_frames, png_frames); parse gives each file's w and h."""
+        """The host form of a multi-file decode (jpeg_frames, png_frames, qoi_frames); parse gives each file's w and h."""
         files, bufs, sizes = _file_args(files)
         geo = [parse(f) for f in files]
         total = sum(g["w"] * g["h"] * 4 for g in geo)
@@ -704,7 +724,7 @@ class Context:
         return canv, status[:len(files)]
 
     def _files_frames_dev(self, fn, files, d_frames, d_status):
-        """The dev form of a multi-file decode (jpeg_frames_dev, png_frames_dev)."""
+        """The dev form of a multi-file decode (jpeg_frames_dev, png_frames_dev, qoi_frames_dev)."""
         import torch
         files, bufs, sizes = _file_args(files)
         if d_status is None:
@@ -729,6 +749,16 @@ class Context:
         """b200timg_png_frames_dev into a device tensor holding every canvas back to back (the src_offset layout of a
         mixed batch): returns d_status, an int32 device tensor with one entry per file, after the (asynchronous) call."""
         return self._files_frames_dev(lib().b200timg_png_frames_dev, files, d_frames, d_status)
+
+    def qoi_frames(self, files):
+        """b200timg_qoi_frames: (list of [h, w, 4] uint8 canvases, int32 status per file) for a list of QOI files;
+        status 2 marks a 3-channel file with alpha below 255, which timg shows uncomposed."""
+        return self._files_frames(lib().b200timg_qoi_frames, qoi_parse, files)
+
+    def qoi_frames_dev(self, files, d_frames, d_status=None):
+        """b200timg_qoi_frames_dev into a device tensor holding every canvas back to back (the src_offset layout of a
+        mixed batch): returns d_status, an int32 device tensor with one entry per file, after the (asynchronous) call."""
+        return self._files_frames_dev(lib().b200timg_qoi_frames_dev, files, d_frames, d_status)
 
     @staticmethod
     def graphics_mixed_bound(b, g):

@@ -1,13 +1,14 @@
-"""Device JPEG or PNG decode (b200timg_jpeg_frames_dev, b200timg_png_frames_dev) against the reference's STB source on
-one host core.
+"""Device JPEG, PNG or QOI decode (b200timg_{jpeg,png,qoi}_frames_dev) against the reference's STB source (JPEG, PNG)
+or QOI source on one host core.
 
 Device time: two CUDA events on the context's stream (also torch's current stream) around the call, recorded after a
 device synchronise, so the upload of the files from pinned staging and every kernel are inside it; the per-kernel split
-comes from ctx.profile in a separate call (png_jump_kernel summed over its rounds).  Reference time: the door onto the
-unmodified STBImageSource (oracle/gif.mk) at capture=0, one decode per file, on the calling thread.  Prints one JSON
+comes from ctx.profile in a separate call (png_jump_kernel and qoi_sync_kernel summed over their rounds).  Reference
+time: the door onto the unmodified STBImageSource (oracle/gif.mk) or QOIImageSource (oracle/qoi.mk) at capture=0, one
+decode per file, on the calling thread.  Prints one JSON
 line per case with the card's name and power limit read in the same run.
 
-    python tools/bench_decode.py --format {jpeg,png} [--steps 5] [--warmup 2] [--ref-steps 1]"""
+    python tools/bench_decode.py --format {jpeg,png,qoi} [--steps 5] [--warmup 2] [--ref-steps 1]"""
 import argparse
 import json
 import os
@@ -23,8 +24,10 @@ import numpy as np  # noqa: E402
 
 import jpeg_cases as jc  # noqa: E402
 import png_cases as pc  # noqa: E402
+import qoi_cases as qc  # noqa: E402
 import timg_b200  # noqa: E402
 from oracle import gif as G  # noqa: E402
+from oracle import qoi as Q  # noqa: E402
 
 
 def jpeg_cases():
@@ -42,7 +45,17 @@ def png_cases():
     yield "thumbs1024_480x270", [pc.pillow(pc.photo(480, 270, k % 16), "RGB") for k in range(1024)]
 
 
-FORMATS = {"jpeg": (jpeg_cases, timg_b200.jpeg_parse, "jpg"), "png": (png_cases, timg_b200.png_parse, "png")}
+def qoi_cases():
+    yield "4k_photo_rgb", [Q.encode(qc.rgba(pc.photo(3840, 2160, 1)), 3)]
+    yield "4k_photo_smooth_rgb", [Q.encode(qc.photo_smooth(3840, 2160, 1), 3)]
+    yield "4k_screenshot_rgb", [Q.encode(qc.rgba(pc.screenshot(3840, 2160, 2)), 3)]
+    yield "4k_gradient_diff_only", [Q.encode(qc.gradient(3840, 2160), 3)]
+    yield "grid64_1080p", [Q.encode(qc.rgba(pc.photo(1920 - 8 * (k % 5), 1080 - 4 * (k % 7), k)), 3) for k in range(64)]
+    yield "thumbs1024_480x270", [Q.encode(qc.rgba(pc.photo(480, 270, k % 16)), 3) for k in range(1024)]
+
+
+FORMATS = {"jpeg": (jpeg_cases, timg_b200.jpeg_parse, "jpg"), "png": (png_cases, timg_b200.png_parse, "png"),
+           "qoi": (qoi_cases, timg_b200.qoi_parse, "qoi")}
 
 
 def main():
@@ -83,7 +96,8 @@ def main():
         prof = {k: round(v[1], 3) for k, v in ctx.profile_report().items() if k.startswith((a.format + "_", "decode_"))}
         ctx.profile(False)
         ref_ms = None
-        if G.have_ref():
+        have_ref, ref_run = (Q.have_ref(), Q.ref_qoi_path) if a.format == "qoi" else (G.have_ref(), G.ref_stb_gif_path)
+        if have_ref:
             with tempfile.TemporaryDirectory() as td:
                 paths = []
                 for i, f in enumerate(files):
@@ -94,7 +108,7 @@ def main():
                 for _ in range(a.ref_steps):
                     t0 = time.perf_counter()
                     for p in paths:
-                        G.ref_stb_gif_path(p, capture=False)
+                        ref_run(p, capture=False)
                     rt.append(time.perf_counter() - t0)
                 ref_ms = 1e3 * float(np.median(rt))
         dev_ms = 1e3 * float(np.median(ts))
