@@ -552,6 +552,55 @@ int b200timg_qoi_frames_dev(b200timg_ctx *ctx, int n_files, const uint8_t *const
 int b200timg_qoi_frames(b200timg_ctx *ctx, int n_files, const uint8_t *const *files, const size_t *sizes,
                         uint8_t *frames, int32_t *status);
 
+/* ======================= BMP, TGA and binary PNM files: the STB source's decode ===================
+ * File f's canvas is the w*h*4 RGBA buffer stbi__load_and_postprocess_8bit(.., 4) gives timg's STB source
+ * (src/stb-image-source.cc:140-157) for a BMP (stbi__bmp_load), TGA (stbi__tga_load) or P5 / P6 PNM (stbi__pnm_load)
+ * file, read from the file as that source reads it, quirks included:
+ *   BMP: bytes past the end read as 0; at 16 bpp and more the gap between the header and bfOffBits is skipped twice; a
+ *     12-byte header has psize (offset - 38) / 3; a 32-bit file with the default masks and every alpha 0 gets alpha
+ *     255; stbi__shiftsigned also takes non-contiguous masks; 1-bpp rows stop mid-byte.
+ *   TGA: the palette starts after tga_palette_start bytes; an index >= the palette's length reads entry 0; 15/16-bit
+ *     grey types decode as RGB16; the right-to-left bit is ignored; RLE packets run across rows and past the image,
+ *     and a stream cut short continues as 1-pixel raw packets of zeros; the BGR swap spares RGB16.
+ *   PNM: 16-bit samples keep their second byte; comments and whitespace as stbi__pnm_skip_whitespace takes them; the
+ *     raster starts right after the character that ends maxval.
+ *
+ * Host only: stb's test and header walk.  B200TIMG_EINVAL exactly where stb's test rejects the file or its load
+ * returns NULL before decoding pixels (bad magic; unknown BMP header size, RLE or JPEG/PNG compression, bad or equal
+ * bitfield masks, masks of more than 8 bits, psize 0 or over 256, stb's "bad offset"; dimensions over 2^24; failed
+ * size checks; a truncated TGA palette; zero or overflowing PNM width or height, maxval over 65535, a truncated PNM
+ * raster).  The BMP, PNM and TGA magics exclude each other and every other format the library decodes, so an adapter
+ * tries the parses in stb's order and falls through on B200TIMG_EINVAL.  supported = 0 (reason says why) where the
+ * reference canvas is not a function of the file: a negative stbi__skip, an uncompressed true-colour TGA cut short, a
+ * 16-bit PNM of 2^28 pixels or more, a zero-area BMP. */
+#define B200TIMG_RASTER_BMP 0
+#define B200TIMG_RASTER_TGA 1
+#define B200TIMG_RASTER_PNM 2
+typedef struct {
+    int format;                      /* B200TIMG_RASTER_* */
+    int w, h;
+    int channels;                    /* stb's channel count (*comp) */
+    int bpp;                         /* bits per pixel: BMP and TGA as the header says, PNM channels * 8 or 16 */
+    int palette;                     /* BMP psize, TGA palette entries, else 0 */
+    int top_down;                    /* 1 when the first row in the file is the top row */
+    int rle;                         /* TGA image types 9-11 */
+    int supported;
+    char reason[96];
+} b200timg_raster_info;
+int b200timg_raster_parse(const uint8_t *data, size_t size, b200timg_raster_info *info);
+/* Canvases of n_files BMP, TGA and PNM files, in any mix, back to back in the src_offset layout of a
+ * b200timg_mixed_batch with B200TIMG_FMT_RGBA.  files: HOST bytes, uploaded in one copy through context-owned pinned
+ * staging.  d_status[f] (device): 1 the canvas is the reference's, and timg composes it like the rest of the page;
+ * -1 a BMP palette index at or past psize reads stb's uninitialised pal[], so the caller decodes the file on the CPU.
+ * B200TIMG_EINVAL before any launch, naming the file: a file b200timg_raster_parse rejects or reports unsupported,
+ * n_files <= 0, d_frames or d_status not 4-byte aligned.  A call launches 7 kernels whatever n_files is and whatever
+ * the files hold. */
+int b200timg_raster_frames_dev(b200timg_ctx *ctx, int n_files, const uint8_t *const *files, const size_t *sizes,
+                               uint8_t *d_frames, int32_t *d_status);
+/* Host form: frames gets the canvases back to back, status[f] as above. */
+int b200timg_raster_frames(b200timg_ctx *ctx, int n_files, const uint8_t *const *files, const size_t *sizes,
+                           uint8_t *frames, int32_t *status);
+
 /* ======================= Kitty / iTerm2 canvases: PNG + base64 (SURVEY 8f rank 2) ===================
  * png::Encode (src/timg-png.cc:90-152): signature, IHDR, one IDAT holding the zlib stream of the scanlines (each
  * row filtered with "Sub"), IEND.  rgb24 != 0: colour type 2 (png::ColorEncoding::kRGB_24), else RGBA.  The

@@ -171,6 +171,9 @@ ABI = {
     "b200timg_qoi_parse": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200timg_qoi_frames_dev": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200timg_qoi_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200timg_raster_parse": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200timg_raster_frames_dev": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200timg_raster_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 _lib = None
@@ -342,6 +345,29 @@ def qoi_parse(data):
     if rc != OK:
         raise B200Error(rc, "qoi_parse: qoi_decode rejects the header")
     return dict(w=info.w, h=info.h, channels=info.channels, colorspace=info.colorspace,
+                supported=bool(info.supported), reason=info.reason.decode())
+
+
+class RasterInfo(C.Structure):
+    _fields_ = [("format", C.c_int), ("w", C.c_int), ("h", C.c_int), ("channels", C.c_int), ("bpp", C.c_int),
+                ("palette", C.c_int), ("top_down", C.c_int), ("rle", C.c_int), ("supported", C.c_int),
+                ("reason", C.c_char * 96)]
+
+
+RASTER_FORMATS = ("bmp", "tga", "pnm")
+
+
+def raster_parse(data):
+    """b200timg_raster_parse (host only) of a BMP, TGA or binary PNM file: a dict of format ('bmp', 'tga' or 'pnm'),
+    w, h, channels, bpp, palette, top_down, rle, supported and reason.  Raises B200Error(EINVAL) where stb's test
+    rejects the file or its load fails before the pixels (so the reference's STB source fails)."""
+    data = bytes(data)
+    info = RasterInfo()
+    rc = lib().b200timg_raster_parse(data, len(data), C.byref(info))
+    if rc != OK:
+        raise B200Error(rc, "raster_parse: stb's header walk fails")
+    return dict(format=RASTER_FORMATS[info.format], w=info.w, h=info.h, channels=info.channels, bpp=info.bpp,
+                palette=info.palette, top_down=bool(info.top_down), rle=bool(info.rle),
                 supported=bool(info.supported), reason=info.reason.decode())
 
 
@@ -759,6 +785,16 @@ class Context:
         """b200timg_qoi_frames_dev into a device tensor holding every canvas back to back (the src_offset layout of a
         mixed batch): returns d_status, an int32 device tensor with one entry per file, after the (asynchronous) call."""
         return self._files_frames_dev(lib().b200timg_qoi_frames_dev, files, d_frames, d_status)
+
+    def raster_frames(self, files):
+        """b200timg_raster_frames: (list of [h, w, 4] uint8 canvases, int32 status per file) for a list of BMP, TGA and
+        PNM files in any mix; status -1 marks a BMP whose canvas reads stb's uninitialised palette."""
+        return self._files_frames(lib().b200timg_raster_frames, raster_parse, files)
+
+    def raster_frames_dev(self, files, d_frames, d_status=None):
+        """b200timg_raster_frames_dev into a device tensor holding every canvas back to back (the src_offset layout of
+        a mixed batch): returns d_status, an int32 device tensor with one entry per file, after the (asynchronous) call."""
+        return self._files_frames_dev(lib().b200timg_raster_frames_dev, files, d_frames, d_status)
 
     @staticmethod
     def graphics_mixed_bound(b, g):

@@ -75,7 +75,9 @@ void b200timg_ctx_destroy(b200timg_ctx *ctx) {
     ctx->out_stage.release(); ctx->offsets.release(); ctx->cells.release(); ctx->rows.release();
     ctx->tables.release(); ctx->sixel_work.release(); ctx->misc.release(); ctx->scale_list.release(); ctx->scale_tmp.release(); ctx->tri_tables.release();
     ctx->mixed_up.release(); ctx->gif_up.release(); ctx->jpeg_up.release(); ctx->png_up.release(); ctx->qoi_up.release();
+    ctx->raster_up.release();
     ctx->gif_scratch.release(); ctx->jpeg_scratch.release(); ctx->png_scratch.release(); ctx->qoi_scratch.release();
+    ctx->raster_scratch.release();
     ctx->pinned.release(); ctx->pinned_io.release();
     ctx->png_sums.release(); ctx->gfx_ids.release();
     ctx->dfl_raw.release(); ctx->dfl_scratch.release(); ctx->dfl_meta.release(); ctx->dfl_tokens.release(); ctx->dfl_png.release();

@@ -133,12 +133,13 @@ struct b200timg_ctx {
     //   GIF decode (gif.cu): file + frame descriptors;
     //   JPEG decode (jpeg.cu): files + descriptors + Huffman tables;
     //   PNG decode (png_decode.cu): files + descriptors;
-    //   QOI decode (qoi.cu): files + descriptors.
-    b200timg::Upload mixed_up, gif_up, jpeg_up, png_up, qoi_up;
+    //   QOI decode (qoi.cu): files + descriptors;
+    //   BMP / TGA / PNM decode (raster.cu): files + descriptors.
+    b200timg::Upload mixed_up, gif_up, jpeg_up, png_up, qoi_up, raster_up;
     // the decoders' per-call scratch: GIF code streams, index planes and per-frame reach; JPEG streams, decoder
     // states, coefficients and planes; PNG zlib streams, raw planes, source indices and copy records; QOI tile maps,
-    // op records and segment states
-    b200timg::DevBuf gif_scratch, jpeg_scratch, png_scratch, qoi_scratch;
+    // op records and segment states; RLE TGA tile maps and packet records
+    b200timg::DevBuf gif_scratch, jpeg_scratch, png_scratch, qoi_scratch, raster_scratch;
 
     int fail(int code, const char *fmt, ...) {
         va_list ap; va_start(ap, fmt);

@@ -1,5 +1,5 @@
-"""Device JPEG, PNG or QOI decode (b200timg_{jpeg,png,qoi}_frames_dev) against the reference's STB source (JPEG, PNG)
-or QOI source on one host core.
+"""Device JPEG, PNG, QOI, BMP, TGA or PNM decode (b200timg_{jpeg,png,qoi,raster}_frames_dev) against the reference's STB
+source (JPEG, PNG, BMP, TGA, PNM) or QOI source on one host core.
 
 Device time: two CUDA events on the context's stream (also torch's current stream) around the call, recorded after a
 device synchronise, so the upload of the files from pinned staging and every kernel are inside it; the per-kernel split
@@ -8,7 +8,7 @@ time: the door onto the unmodified STBImageSource (oracle/gif.mk) or QOIImageSou
 decode per file, on the calling thread.  Prints one JSON
 line per case with the card's name and power limit read in the same run.
 
-    python tools/bench_decode.py --format {jpeg,png,qoi} [--steps 5] [--warmup 2] [--ref-steps 1]"""
+    python tools/bench_decode.py --format {jpeg,png,qoi,bmp,tga,pnm} [--steps 5] [--warmup 2] [--ref-steps 1]"""
 import argparse
 import json
 import os
@@ -25,9 +25,11 @@ import numpy as np  # noqa: E402
 import jpeg_cases as jc  # noqa: E402
 import png_cases as pc  # noqa: E402
 import qoi_cases as qc  # noqa: E402
+import raster_cases as rc  # noqa: E402
 import timg_b200  # noqa: E402
 from oracle import gif as G  # noqa: E402
 from oracle import qoi as Q  # noqa: E402
+from oracle import raster as R  # noqa: E402
 
 
 def jpeg_cases():
@@ -54,8 +56,35 @@ def qoi_cases():
     yield "thumbs1024_480x270", [Q.encode(qc.rgba(pc.photo(480, 270, k % 16)), 3) for k in range(1024)]
 
 
+def _grid_photos():
+    return [pc.photo(1920 - 8 * (k % 5), 1080 - 4 * (k % 7), k) for k in range(64)]
+
+
+def bmp_cases():
+    yield "4k_photo_24", [R.bmp(pc.photo(3840, 2160, 1), 24)]
+    yield "grid64_1080p", [R.bmp(p, 24) for p in _grid_photos()]
+    yield "thumbs1024_480x270", [R.bmp(pc.photo(480, 270, k % 16), 24) for k in range(1024)]
+
+
+def tga_cases():
+    for rle in (False, True):
+        tag = "rle" if rle else "raw"
+        yield f"4k_photo_{tag}", [rc.tga_file(pc.photo(3840, 2160, 1), rle)]
+        yield f"4k_screenshot_{tag}", [rc.tga_file(pc.screenshot(3840, 2160, 2), rle)]
+        yield f"grid64_1080p_{tag}", [rc.tga_file(p, rle) for p in _grid_photos()]
+        yield f"thumbs1024_480x270_{tag}", [rc.tga_file(pc.photo(480, 270, k % 16), rle) for k in range(1024)]
+
+
+def pnm_cases():
+    yield "4k_photo_p6", [R.pnm(pc.photo(3840, 2160, 1))]
+    yield "grid64_1080p", [R.pnm(p) for p in _grid_photos()]
+    yield "thumbs1024_480x270", [R.pnm(pc.photo(480, 270, k % 16)) for k in range(1024)]
+
+
 FORMATS = {"jpeg": (jpeg_cases, timg_b200.jpeg_parse, "jpg"), "png": (png_cases, timg_b200.png_parse, "png"),
-           "qoi": (qoi_cases, timg_b200.qoi_parse, "qoi")}
+           "qoi": (qoi_cases, timg_b200.qoi_parse, "qoi"), "bmp": (bmp_cases, timg_b200.raster_parse, "bmp"),
+           "tga": (tga_cases, timg_b200.raster_parse, "tga"), "pnm": (pnm_cases, timg_b200.raster_parse, "ppm")}
+RASTER = ("bmp", "tga", "pnm")
 
 
 def main():
@@ -72,7 +101,8 @@ def main():
     ctx = timg_b200.Context(0, stream=stream.cuda_stream)
     torch.cuda.set_stream(stream)
     cases, parse, ext = FORMATS[a.format]
-    frames_dev = getattr(ctx, f"{a.format}_frames_dev")
+    frames_dev = getattr(ctx, "raster_frames_dev" if a.format in RASTER else f"{a.format}_frames_dev")
+    prefixes = ("tga_", "raster_") if a.format in RASTER else (a.format + "_", "decode_")
     for name, files in cases():
         geo = [parse(f) for f in files]
         rgba = sum(g["w"] * g["h"] * 4 for g in geo)
@@ -93,7 +123,7 @@ def main():
         ctx.profile(True)
         frames_dev(files, d)
         torch.cuda.synchronize()
-        prof = {k: round(v[1], 3) for k, v in ctx.profile_report().items() if k.startswith((a.format + "_", "decode_"))}
+        prof = {k: round(v[1], 3) for k, v in ctx.profile_report().items() if k.startswith(prefixes)}
         ctx.profile(False)
         ref_ms = None
         have_ref, ref_run = (Q.have_ref(), Q.ref_qoi_path) if a.format == "qoi" else (G.have_ref(), G.ref_stb_gif_path)
